@@ -202,9 +202,10 @@ int LizardB200_compress_device(const void* dSrc, const uint64_t* dSrcOff, const 
  * packs the units of a batch back to back.  Enqueue-only, like the calls above. */
 int LizardB200_gather_device(const void* dSrc, const uint64_t* dSrcOff, const int* dLen,
                              void* dDst, const uint64_t* dDstOff, unsigned nUnits, void* cudaStream);
-/* diagnostics: default launch shape of the encode kernel for a level (no device needed): warps per CTA, how many of them
- * keep their hash table in shared memory, CTAs per SM, dynamic shared memory per CTA.  LIZARDB200_ERR_LEVEL for levels
- * whose parser is not implemented. */
+/* diagnostics: launch shape of the encode kernel for a level (no device needed): warps per CTA, how many of them keep their
+ * hash table in shared memory, CTAs per SM (an upper bound: a launch holds no more than fit), dynamic shared memory per CTA.
+ * The level's default, or LIZARDB200_ENC_SHAPE="warps,tables,ctas" when that is set and valid, exactly as the encoder
+ * launches it.  LIZARDB200_ERR_LEVEL for levels whose parser is not implemented. */
 int LizardB200_encodeShape(int compressionLevel, int* warpsPerCta, int* smemTables, int* ctasPerSM, int* smemBytes);
 /* diagnostics (no device needed): pipeline chunk of a unit in a host-buffer call of nUnits units with unitsPerChunk units per
  * chunk (ramp != 0: the decoder's doubling ramp of small first chunks), computed by the host code and by the kernels'

@@ -568,13 +568,13 @@ int LizardB200_available(void)
 const char* LizardB200_lastError(void) { return g_last_error.c_str(); }
 unsigned long long LizardB200_launchCount(void) { return g_launches.load(); }
 
-// diagnostics: the encode kernel's default launch shape for a level (pure host arithmetic, needs no device): warps per CTA,
-// how many of them keep their hash table in shared memory, CTAs per SM, dynamic shared bytes per CTA
+// diagnostics: the encode kernel's launch shape for a level, LIZARDB200_ENC_SHAPE applied (pure host arithmetic, needs no
+// device): warps per CTA, how many of them keep their hash table in shared memory, CTAs per SM, dynamic shared bytes per CTA
 int LizardB200_encodeShape(int level, int* warpsPerCta, int* smemTables, int* ctasPerSM, int* smemBytes)
 {
     const LevelParams lp = level_params(level);
     if (lp.parser == kParserUnsupported) return LIZARDB200_ERR_LEVEL;
-    const EncodeShape sh = encode_shape(lp);
+    const EncodeShape sh = encode_shape_in_effect(lp);
     if (warpsPerCta) *warpsPerCta = sh.warps;
     if (smemTables) *smemTables = sh.smem_tables;
     if (ctasPerSM) *ctasPerSM = sh.ctas_per_sm;

@@ -266,17 +266,26 @@ inline EncodeShape encode_shape(const LevelParams& lp)
     return best;
 }
 
-inline cudaError_t encode_launch(const EncodeConfig& c, const EncodeBatch& b, cudaStream_t s, int* launches)
+// The shape a launch uses: encode_shape(), unless LIZARDB200_ENC_SHAPE="warps,tables,ctas" is set and valid (diagnostics and
+// tests: "14,0,2" runs every warp on the plain global table, "1,1,1" one warp per SM on a shared-memory table).  Levels
+// without a shared-memory table keep 0 tables whatever the variable asks.  The CTAs per SM are an upper bound the launch
+// lowers to what the device can hold.
+inline EncodeShape encode_shape_in_effect(const LevelParams& lp)
 {
-    const LevelParams lp = level_params(b.level);
     EncodeShape sh = encode_shape(lp);
-    if (const char* e = getenv("LIZARDB200_ENC_SHAPE")) {           // diagnostics: "warps,tables,ctas"
+    if (const char* e = getenv("LIZARDB200_ENC_SHAPE")) {
         int w = 0, t = 0, k = 0;
         if (sscanf(e, "%d,%d,%d", &w, &t, &k) == 3 && w >= 1 && w <= kEncWarpsPerCta && t >= 0 && t <= w && k >= 1) {
             sh.warps = w; sh.smem_tables = sh.table_bytes ? t : 0; sh.ctas_per_sm = k;
             sh.smem = (size_t)sh.smem_tables * sh.table_bytes + (size_t)w * sh.hist_bytes;
         }
     }
+    return sh;
+}
+
+inline cudaError_t encode_launch(const EncodeConfig& c, const EncodeBatch& b, cudaStream_t s, int* launches)
+{
+    const EncodeShape sh = encode_shape_in_effect(level_params(b.level));
     const size_t per_warp = c.per_warp_small;
     int per_sm = 0;
     // the occupancy query honours the kernel's current carve-out preference, which the previous launch (possibly of

@@ -1,0 +1,442 @@
+"""Input corpus shared by the CPU and GPU suites, and a plain-Python walker of Lizard streams.
+
+The families are built to reach the edges of the format where a codec goes wrong: matches 65536 or more bytes back (the
+24-bit-offset codewords and the LIZv1 parsers' far-candidate rule), literal runs and matches of exact lengths at every
+boundary between the length-extension widths, Huffman-hostile literal alphabets, and periodic data whose periods straddle
+the decoder's wide-copy threshold.  `walk` decodes streams without a Huffman stage and counts the codeword classes it
+met, so the tests can prove that the corpus really reaches what it claims to."""
+import random
+from collections import Counter
+
+import numpy as np
+
+import lizard_b200 as lz
+
+BS = lz.BLOCK_SIZE
+MINMATCH = 4
+MM_LONGOFF = 16                 # LIZv1: a 24-bit-offset match is at least this long
+LAST_LONG_OFF = 31              # LIZv1 token 31: 24-bit offset, match length 47 + extension
+MAX_16BIT_OFFSET = 1 << 16
+
+# literal run / match lengths at the boundaries between the 0-, 1-, 3- and 4-byte extension forms
+#   LZ4 codewords: token field 15, then one byte, 254 + LE16 from 15 + 254, 255 + LE24 from 15 + 65536
+#   LIZv1 codewords: literals 7 / 7 + 254 / 7 + 65536, matches 15 / 15 + 254 / 15 + 65536
+LZ4_LITERALS = (14, 15, 16, 268, 269, 270, 65550, 65551)
+LZ4_MATCHES = tuple(MINMATCH + n for n in (14, 15, 16, 268, 269, 270, 65550, 65551))
+LIZ_LITERALS = (6, 7, 8, 260, 261, 65542, 65543)
+LIZ_MATCHES = (14, 15, 16, 268, 269, 65550, 65551)
+# 24-bit-offset matches: shorter than MM_LONGOFF + MINMATCH (refused by the far-candidate rule), token 0-30 (16-46),
+# token 31 with a zero / one-byte / 254 + LE16 extension (47, 48, 300, 301)
+FAR_LENGTHS = (15, 16, 17, 19, 20, 46, 47, 48, 300, 301)
+PERIODS = (8, 9, 15, 16, 17, 31, 32, 33, 64, 100, 255, 256, 257, 511, 512, 543, 544, 545, 600)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# families kept from the first CPU suite (same seeds, same bytes)
+# ---------------------------------------------------------------------------------------------------------------------
+def far_match_input(seed=3, n=BS):
+    """Matches 65536 or more bytes back, short and long: exercises the LIZv1 parsers' rule that a far candidate is only taken
+    when the match is at least MM_LONGOFF + MINMATCH long (lizard_parser_fastbig.h:99,142; lizard_parser_pricefast.h:69) and
+    the 24-bit-offset codewords."""
+    rnd = random.Random(seed)
+    head = bytes(rnd.randrange(256) for _ in range(70000))
+    out = bytearray(head)
+    while len(out) < n:
+        k = rnd.choice([5, 8, 12, 17, 19, 20, 21, 24, 40, 100])
+        at = rnd.randrange(0, 4000)                      # source near the start: offsets >= 65536
+        out += head[at:at + k]
+        out += bytes(rnd.randrange(256) for _ in range(rnd.randrange(1, 30)))
+    return bytes(out[:n])
+
+
+def inputs(seed, count):
+    """Mixed sizes (0 to 200000 bytes) and kinds: datagen, zeros, uniform random, 4-letter alphabet, a repeated 8-byte
+    pattern, a skewed 4-symbol alphabet, Dirichlet(0.05) bytes."""
+    rnd = random.Random(seed)
+    rng = np.random.default_rng(seed)
+    out = []
+    for _ in range(count):
+        kind = rnd.randrange(7)
+        n = rnd.choice([0, 1, 5, 19, 20, 21, 22, 40, 100, 1000, 1025, 2000, 4096, 30000, 65536, 131071, 131072,
+                        131073, 200000])
+        if kind == 0:
+            out.append(lz.datagen(n, rnd.choice([10, 30, 50, 70, 90, 100]), rnd.randrange(1000)))
+        elif kind == 1:
+            out.append(bytes(n))
+        elif kind == 2:
+            out.append(rng.integers(0, 256, n, dtype=np.uint8).tobytes())
+        elif kind == 3:
+            out.append(rng.integers(0, 4, n, dtype=np.uint8).tobytes())
+        elif kind == 4:
+            out.append((b"abcdefgh" * (n // 8 + 1))[:n])
+        elif kind == 5:
+            out.append(rng.choice(np.array([65, 66, 67, 200], dtype=np.uint8), size=n, p=[0.9, 0.05, 0.04, 0.01]).tobytes())
+        else:
+            p = rng.dirichlet(np.ones(256) * 0.05)
+            out.append(rng.choice(256, size=n, p=p).astype(np.uint8).tobytes())
+    return out
+
+
+def skewed(rnd, n, nrare, tail):
+    """Three common symbols (97 %) and `nrare` rare ones; the last `tail` share of the block is mostly rare symbols, so the
+    Huffman codes of its literals are long (10/11 bits) where the stream ends."""
+    common = [rnd.randrange(256) for _ in range(3)]
+    rare = rnd.sample(range(256), nrare)
+    out = bytearray()
+    cut = int(n * (1 - tail))
+    while len(out) < cut:
+        out.append(rnd.choice(common) if rnd.random() < 0.97 else rnd.choice(rare))
+    while len(out) < n:
+        out.append(rnd.choice(rare) if rnd.random() < 0.9 else rnd.choice(common))
+    return bytes(out)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# new families
+# ---------------------------------------------------------------------------------------------------------------------
+def _random(rng, n):
+    return rng.integers(0, 256, n, dtype=np.uint8).tobytes()
+
+
+def far_unit(seed, n=BS, head=70000):
+    """`head` fresh random bytes, then copies of FAR_LENGTHS bytes from the head, each at least 65536 bytes back, with and
+    without literals before them.  Every copy takes its own part of the head, and the bytes around a copy differ from the
+    bytes around its source, so each copy is one match of exactly its length (or literals, when the parser refuses it)."""
+    rnd = random.Random(seed)
+    rng = np.random.default_rng(seed)
+    src = _random(rng, head)
+    out = bytearray(src)
+    cur = 1                                             # next unused byte of the head
+    cont = None                                         # the byte that would continue the previous copy's match
+    lengths = FAR_LENGTHS + ((2000, 65583, 65584) if n > 2 * head else ())     # 65583 = 47 + 65536: 4-byte extension
+    while True:
+        k = rnd.choice(lengths)
+        gap = rnd.choice([0, 0, 1, 2, 5, 7, 8, 30])
+        at = cur + 1
+        if gap == 0:                                    # neither end may continue the previous copy
+            while at + k < head and (src[at] == cont or src[at - 1] == out[-1]):
+                at += 1
+        if len(out) + gap + k + 64 > n or at + k + 1 > head:
+            break
+        assert len(out) + gap - at >= MAX_16BIT_OFFSET
+        if gap:
+            lit = bytearray(_random(rng, gap))
+            while lit[0] == cont or lit[-1] == src[at - 1]:
+                lit[0], lit[-1] = rnd.randrange(256), rnd.randrange(256)
+            out += lit
+        out += src[at:at + k]
+        cont = src[at + k]
+        cur = at + k + 1
+    tail = bytearray(_random(rng, n - len(out)))
+    if tail and tail[0] == cont:
+        tail[0] ^= 0x5A
+    return bytes(out + tail)
+
+
+def far_units(seed=40):
+    """Single-block units (128 KiB) and multi-inner-block units (1.5 and 3 MiB) whose copies reach more than 1 MiB back."""
+    return [far_unit(seed, BS), far_unit(seed + 1, BS), far_unit(seed + 2, BS - 777),
+            far_unit(seed + 3, 3 * (1 << 19), head=1100000), far_unit(seed + 4, 3 << 20, head=1200000)]
+
+
+def threshold_unit(seed, literals, matches, n=BS, head=16384):
+    """Fresh random literal runs and copied matches of exactly the given lengths, (literals, match) pairs taken in turn
+    until the unit is full.  A match copies from inside its own literal run (off <= run; off < length makes the match
+    periodic) or, behind runs shorter than 8 bytes and for the long matches, from an unused part of a random head.  The
+    last literal and the byte behind the match differ from the bytes around the source, so a match cannot grow."""
+    rnd = random.Random(seed)
+    rng = np.random.default_rng(seed)
+    out = bytearray(_random(rng, head))
+    hcur = 1                                            # next unused byte of the head
+    cont = None
+    pairs = [(a, b) for a in literals for b in matches]
+    rnd.shuffle(pairs)
+    misses = 0
+    for lit, ml in (pairs[i % len(pairs)] for i in range(1 << 30)):
+        if misses > len(pairs):
+            break
+        pos = len(out) + lit
+        if pos + ml + 64 > n:
+            misses += 1
+            continue
+        if ml > 2000:
+            off = rnd.choice([1000, 4096, 9999])
+            if pos - off < hcur or len(out) != head:        # the only pair of its unit: the source is the head's end
+                misses += 1
+                continue
+        elif lit >= 8:
+            off = rnd.randrange(8, lit + 1)
+        else:
+            off = pos - hcur
+            if off >= 60000 or hcur + ml + 1 > head:
+                misses += 1
+                continue
+            hcur += ml + 2
+        misses = 0
+        run = bytearray(_random(rng, lit))
+        if lit:
+            while run[0] == cont or run[-1] == (out[pos - 1 - off] if pos - 1 - off < len(out) else run[pos - 1 - off - len(out)]):
+                run[0], run[-1] = rnd.randrange(256), rnd.randrange(256)
+        out += run
+        for _ in range(ml):
+            out.append(out[-off])
+        cont = out[-off]
+    tail = bytearray(_random(rng, n - len(out)))
+    if tail and tail[0] == cont:
+        tail[0] ^= 0x5A
+    return bytes(out + tail)
+
+
+def threshold_units(seed=50):
+    """Per flavour: one block of the short boundaries, and blocks that hold one 64 KiB+ literal run or match followed by a
+    copy, so that the block still compresses."""
+    short = lambda xs: tuple(x for x in xs if x < 1000)
+    long_ = lambda xs: tuple(x for x in xs if x > 60000)
+    out = []
+    for k, (lits, mls) in enumerate(((LZ4_LITERALS, LZ4_MATCHES), (LIZ_LITERALS, LIZ_MATCHES))):
+        s = seed + 10 * k
+        out.append(threshold_unit(s, short(lits), short(mls)))
+        for j, ll in enumerate(long_(lits)):        # a 64 KiB+ run, then a long copy of part of it
+            out.append(threshold_unit(s + 1 + j, (ll,), (40000,), head=0))
+        for j, ml in enumerate(long_(mls)):         # a 64 KiB+ match (periodic) behind a short literal run
+            out.append(threshold_unit(s + 5 + j, short(lits)[:1], (ml,)))
+    return out
+
+
+def hostile_units(seed=60):
+    """Literal alphabets the Huffman stage finds hard: many rare symbols (code lengths at the 11-bit limit), a skewed
+    block whose stream ends in rare symbols, one symbol (RLE streams) and two symbols (nearly incompressible literals or a
+    stored stream)."""
+    rnd = random.Random(seed)
+    rng = np.random.default_rng(seed)
+    p = np.concatenate([np.full(4, 0.24), rng.dirichlet(np.ones(252) * 0.3) * 0.04])
+    rare = rng.choice(256, size=BS, p=p).astype(np.uint8).tobytes()
+    dirichlet = rng.choice(256, size=BS - 5, p=rng.dirichlet(np.ones(256) * 0.02)).astype(np.uint8).tobytes()
+    two = rng.choice(np.array([0x31, 0xC7], dtype=np.uint8), size=70000, p=[0.5, 0.5]).tobytes()
+    two_skew = rng.choice(np.array([0x00, 0xFF], dtype=np.uint8), size=BS, p=[0.995, 0.005]).tobytes()
+    return [rare, dirichlet, skewed(rnd, BS, 200, 0.1), bytes([0x41]) * BS, two, two_skew]
+
+
+def periodic_units(seed=70, n=20000):
+    """A random period of PERIODS bytes repeated, with a byte changed every few thousand bytes: long overlapping matches at
+    offsets on both sides of the decoder's wide-copy threshold, and (LIZv1) repeat offsets after each change."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for p in PERIODS:
+        base = bytearray((_random(rng, p) * (n // p + 1))[:n])
+        for at in rng.integers(100, n, size=n // 3000):
+            base[int(at)] ^= 0xA5
+        out.append(bytes(base))
+    return out
+
+
+def corpus():
+    """family -> list of units (about 6 MiB in all)."""
+    return {"far": far_units(), "threshold": threshold_units(), "hostile": hostile_units(), "periodic": periodic_units()}
+
+
+def edge_capacities(rnd, units, bound):
+    """Destination capacities drawn like the GPU edge-input test: the bound twice, one byte short of the input, half of it
+    plus one, anything from 1 to the bound."""
+    return [rnd.choice([bound(len(u)), bound(len(u)), max(len(u) - 1, 1), len(u) // 2 + 1, rnd.randrange(1, bound(len(u)) + 1)])
+            for u in units]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# walker
+# ---------------------------------------------------------------------------------------------------------------------
+def _le(b, at, n):
+    if at + n > len(b):
+        raise ValueError("stream ends inside a field")
+    return int.from_bytes(b[at:at + n], "little")
+
+
+def is_lizv1(level):
+    return 20 <= level <= 29 or 40 <= level <= 49
+
+
+class _Stream:
+    def __init__(self, data):
+        self.b, self.p = data, 0
+
+    def byte(self):
+        if self.p >= len(self.b):
+            raise ValueError("stream exhausted")
+        self.p += 1
+        return self.b[self.p - 1]
+
+    def take(self, n):
+        if self.p + n > len(self.b):
+            raise ValueError("stream exhausted")
+        self.p += n
+        return self.b[self.p - n:self.p]
+
+    def ext(self, classes, kind):
+        """One length extension: a byte, 254 + LE16 or 255 + LE24 (lizard_decompress_lz4.h:48-64)."""
+        v = self.byte()
+        if v == 254:
+            classes[kind + "_ext3"] += 1
+            return _le(self.take(2), 0, 2)
+        if v == 255:
+            classes[kind + "_ext4"] += 1
+            return _le(self.take(3), 0, 3)
+        classes[kind + "_ext1"] += 1
+        return v
+
+
+def _copy(out, off, n):
+    if off < 1 or off > len(out):
+        raise ValueError("offset %d outside the output (%d bytes)" % (off, len(out)))
+    if off >= n:
+        out += out[len(out) - off:len(out) - off + n]
+    else:                                               # overlapping: the last `off` bytes repeat
+        out += (out[-off:] * (n // off + 1))[:n]
+
+
+def walk(comp):
+    """Decode a Lizard stream whose inner blocks carry no Huffman-coded stream (levels 10-29, or blocks of the higher levels
+    the encoder stored plain), following Lizard_decompress_generic (lib/lizard_decompress.c:115-264; streams as read by
+    Lizard_readStream, :72-112).  Returns (decoded bytes, Counter of codeword classes):
+      lit_ext0/1/3/4, match_ext0/1/3/4   width in bytes of a length's extension (0: the length fits the token)
+      off16, off24, off_repeat           how a match's offset was coded
+      far_short, far_long                LIZv1 24-bit-offset tokens 0-30 and 31
+      far_after_literals                 a far token behind a literal-only token (literals before a far match)
+      raw_block, block                   stored and coded inner blocks
+      ("lit", n), ("match", n), ("far", n)   lengths of literal runs, of 16-bit/repeat matches and of far matches.
+    Raises ValueError on a stream the reference would refuse (as far as a valid-stream walker needs to tell)."""
+    if not comp:
+        raise ValueError("empty input")
+    level = comp[0]
+    if not 10 <= level <= 49:
+        raise ValueError("level %d" % level)
+    lizv1 = is_lizv1(level)
+    out = bytearray()
+    classes = Counter()
+    ip = 1
+    while ip < len(comp):
+        flag = comp[ip]
+        ip += 1
+        if flag == 0x80:
+            n = _le(comp, ip, 3)
+            ip += 3
+            if ip + n > len(comp):
+                raise ValueError("raw block past the end")
+            out += comp[ip:ip + n]
+            ip += n
+            classes["raw_block"] += 1
+            continue
+        if flag & 16:
+            raise ValueError("flag 0x%x" % flag)
+        if flag & 15:
+            raise NotImplementedError("Huffman-coded stream (flag 0x%x)" % flag)
+        streams = []
+        for _ in range(5):                              # lengths (unused by the decoder), off16, off24, flags, literals
+            n = _le(comp, ip, 3)
+            if ip + 3 + n > len(comp):
+                raise ValueError("stream past the end")
+            streams.append(comp[ip + 3:ip + 3 + n])
+            ip += 3 + n
+        classes["block"] += 1
+        _, off16, off24, flags, lits = (_Stream(s) for s in streams)
+        (_block_liz if lizv1 else _block_lz4)(out, flags, lits, off16, off24, classes)
+        if lits.p != len(lits.b):                       # last literals: the rest of the stream
+            n = len(lits.b) - lits.p
+            out += lits.take(n)
+    return bytes(out), classes
+
+
+def _block_lz4(out, flags, lits, off16, off24, classes):
+    while flags.p < len(flags.b):
+        token = flags.byte()
+        n = token & 15
+        if n == 15:
+            n = 15 + lits.ext(classes, "lit")
+        else:
+            classes["lit_ext0"] += 1
+        classes[("lit", n)] += 1
+        out += lits.take(n)
+        off = _le(lits.take(2), 0, 2)
+        classes["off16"] += 1
+        ml = token >> 4
+        if ml == 15:
+            ml = 15 + lits.ext(classes, "match")
+        else:
+            classes["match_ext0"] += 1
+        ml += MINMATCH
+        classes[("match", ml)] += 1
+        _copy(out, off, ml)
+
+
+def _block_liz(out, flags, lits, off16, off24, classes):
+    last_off = 0                                        # LIZARD_INIT_LAST_OFFSET, per inner block
+    lit_only = False
+    while flags.p < len(flags.b):
+        token = flags.byte()
+        if token >= 32:
+            n = token & 7
+            if n == 7:
+                n = 7 + lits.ext(classes, "lit")
+            else:
+                classes["lit_ext0"] += 1
+            classes[("lit", n)] += 1
+            out += lits.take(n)
+            if token >> 7:
+                if (token >> 3) & 15:
+                    classes["off_repeat"] += 1
+            else:
+                last_off = _le(off16.take(2), 0, 2)
+                classes["off16"] += 1
+            ml = (token >> 3) & 15
+            if ml == 15:
+                ml = 15 + lits.ext(classes, "match")
+            else:
+                classes["match_ext0"] += 1
+            lit_only = ml == 0
+            if ml:
+                classes[("match", ml)] += 1
+                _copy(out, last_off, ml)
+            continue
+        if token < LAST_LONG_OFF:
+            ml = token + MM_LONGOFF
+            classes["far_short"] += 1
+        else:
+            ml = lits.ext(classes, "match") + LAST_LONG_OFF + MM_LONGOFF
+            classes["far_long"] += 1
+        if lit_only:
+            classes["far_after_literals"] += 1
+        lit_only = False
+        last_off = _le(off24.take(3), 0, 3)
+        classes["off24"] += 1
+        classes[("far", ml)] += 1
+        _copy(out, last_off, ml)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# what the corpus must reach
+# ---------------------------------------------------------------------------------------------------------------------
+ENCODE_LEVELS = [10, 11, 13, 14, 15, 16, 17, 20, 21, 22, 30, 31, 34, 35, 36, 37, 38, 40, 41, 42]     # implemented on the GPU
+WALKED_ENCODE_LEVELS = [lv for lv in ENCODE_LEVELS if lv < 30]                                     # no Huffman stage
+
+
+def targets(family, lizv1):
+    """Codeword classes (walk's names) that a family's streams must contain, summed over the walked encode levels of one
+    codeword flavour."""
+    if family == "threshold":
+        lits, mls = (LIZ_LITERALS, LIZ_MATCHES) if lizv1 else (LZ4_LITERALS, LZ4_MATCHES)
+        return ({k + "_ext" + w for k in ("lit", "match") for w in "0134"} | {"off16"}
+                | {("lit", n) for n in lits} | {("match", n) for n in mls})
+    if family == "far":
+        if not lizv1:                                   # 64 KiB window: the far copies stay literals, the heads raw blocks
+            return {"raw_block"}
+        return ({"raw_block", "off24", "off_repeat", "far_short", "far_long", "far_after_literals", "match_ext1", "match_ext3",
+                 "match_ext4"} | {("far", n) for n in (20, 46, 47, 48, 300, 301, 65583, 65584)})
+    if family == "periodic":
+        return {"off16", "match_ext3"} | ({"off_repeat"} if lizv1 else set())
+    if family == "hostile":
+        return {"off16", "match_ext4"}
+    raise KeyError(family)
+
+
+def missing(family, lizv1, classes):
+    """The targets of a family that `classes` lacks, by name."""
+    return sorted((t for t in targets(family, lizv1) if classes[t] == 0), key=str)

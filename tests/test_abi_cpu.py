@@ -149,6 +149,39 @@ def test_encoder_launch_shapes_are_the_measured_ones():
     assert L.LizardB200_encodeShape(12, None, None, None, None) < 0
 
 
+def test_encoder_launch_shape_override_is_reported():
+    """LIZARDB200_ENC_SHAPE="warps,tables,ctas" forces the encoder's launch shape; LizardB200_encodeShape reports what the
+    encoder will launch (the same parsing), so tests can confirm the override took effect.  Levels without a shared-memory
+    table keep 0 tables; malformed or out-of-range values leave the measured shape."""
+    import subprocess
+    import sys
+    prog = ("import ctypes, lizard_b200 as lz\n"
+            "L = lz.lib()\n"
+            "for level in (10, 21, 11, 41):\n"
+            "    v = [ctypes.c_int() for _ in range(4)]\n"
+            "    assert L.LizardB200_encodeShape(level, *[ctypes.byref(x) for x in v]) == 0\n"
+            "    print(level, *[x.value for x in v])\n")
+    def shapes(value):
+        env = dict(os.environ)
+        env.pop("LIZARDB200_ENC_SHAPE", None)
+        if value is not None:
+            env["LIZARDB200_ENC_SHAPE"] = value
+        r = subprocess.run([sys.executable, "-c", prog], cwd=ROOT, env=env, capture_output=True, text=True, timeout=120)
+        assert r.returncode == 0, r.stderr
+        return {int(f[0]): tuple(int(x) for x in f[1:]) for f in map(str.split, r.stdout.strip().splitlines())}
+    default = shapes(None)
+    assert {lv: s[:3] for lv, s in default.items()} == {10: (14, 7, 2), 21: (14, 2, 2), 11: (14, 0, 2), 41: (14, 1, 2)}
+    plain = shapes("14,0,2")
+    assert all(s[:3] == (14, 0, 2) for s in plain.values()), plain
+    assert plain[41][3] == 14 * 4096 and plain[10][3] == 0           # the Huffman levels keep their per-warp histograms
+    solo = shapes("1,1,8")
+    assert solo[10][:3] == (1, 1, 8) and solo[21][:3] == (1, 1, 8) and solo[41][:3] == (1, 1, 8)
+    assert solo[11][:3] == (1, 0, 8)                                   # hashLog 18: no shared-memory table to give
+    assert solo[41][3] == solo[21][3] + 4096 and solo[21][3] > 0       # one table; level 41 adds its histograms
+    for bad in ("15,1,2", "2,3,1", "0,0,1", "14,0,0", "14,0", "x"):
+        assert shapes(bad) == default, bad
+
+
 def test_pipeline_chunk_plan_host_and_kernel_arithmetic_agree():
     """The host-buffer calls cut their units into pipeline chunks (frame.inl: FrameChunks; the decoder's calls start with a
     doubling ramp of small chunks); the kernels find a unit's chunk with their own arithmetic (decode.cuh: progress_chunk).
