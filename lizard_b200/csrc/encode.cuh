@@ -1,6 +1,11 @@
 // encode.cuh -- device kernel around encode_core.cuh: one warp per independent unit
 // (= one Lizard_compress call, normally one 128 KiB frame block), persistent grid, atomic work queue.
 //
+// The kernel is one template, lizard_encode_units_kernel<kFam>, instantiated per parser family (enc_family() in
+// encode_core.cuh): Fast (levels 10/11: 72 registers, no stack), FastBig (20) and Generic (the rest, Huffman stage
+// included).  Every instance has the same launch bounds, table setup and frame packing; encode_launch() runs the level's.
+// Level 10 on an H100 SXM 80 GB at a 400 W limit: 11.7 ms per GiB (12.2 with one kernel for all levels).
+//
 // Memory placement per warp (launch shape per level: encode_shape() below):
 //   shared : the PACKED hash table (16-bit entries + a bit plane for position bit 16 + one tag byte per entry for the fast
 //            parsers: 12.5 KiB at level 10/30, 34 KiB untagged at 20/21/40/41) for as many of a CTA's 14 warps as the
@@ -160,33 +165,18 @@ constexpr int kEncWarpsPerCta = 14, kEncCtasPerSM = 2, kEncMaxWarpsPerSM = kEncW
 #if !defined(LZB_ENC_OPAQUE)
 #define LZB_ENC_OPAQUE 2
 #endif
+// One instance per parser family (enc_family(), encode_core.cuh); the launch picks the level's instance.
+template <int kFam>
 __global__ void __launch_bounds__(32 * kEncWarpsPerCta, kEncCtasPerSM)
 lizard_encode_units_kernel(EncodeBatch b, u32 smem_tables, u32 table_bytes, u32 hist_bytes, size_t per_warp_bytes)
 {
     extern __shared__ __align__(16) unsigned char enc_smem[];
     const u32 lane = WarpLanes::lane(), wic = threadIdx.x >> 5, wpc = blockDim.x >> 5;
-    u8* my = b.scratch + ((size_t)blockIdx.x * wpc + wic) * per_warp_bytes;
-#if LZB_ENC_OPAQUE
-    // the warp's scratch base and table base stay in registers: left to itself the compiler re-derives them (a 64-bit
-    // multiply-add) in front of every access
-    asm volatile("" : "+l"(my));
-#endif
-    EncWork* work = reinterpret_cast<EncWork*>(my);
+    const size_t my_off = ((size_t)blockIdx.x * wpc + wic) * per_warp_bytes;
     // shared layout: [smem_tables packed hash tables][per-warp 4 KiB segment histograms, entropy levels only]
-    const LevelParams klp = level_params(b.level);
     const bool packed_ok = wic < smem_tables;
-    u8* tab = enc_smem + (size_t)wic * table_bytes;
-#if LZB_ENC_OPAQUE >= 2
-    asm volatile("" : "+l"(tab));                // (generic instead of shared-space accesses to the packed table then)
-#endif
     u32* seg_hist = reinterpret_cast<u32*>(enc_smem + (size_t)smem_tables * table_bytes + (size_t)wic * hist_bytes);
-    const bool tagged = enc_tagged(klp), tagged_plain = enc_tagged_plain(klp);
-    HashTable packed, plain;
-    packed.t32 = nullptr; packed.lo = reinterpret_cast<u16*>(tab);
-    packed.hi = reinterpret_cast<u32*>(tab + ((size_t)2 << klp.hashLog));
-    packed.tag = tagged ? tab + hash_packed_bytes(klp.hashLog, false) : nullptr; packed.tagged = 0;
-    plain.t32 = reinterpret_cast<u32*>(my + sizeof(EncWork)); plain.lo = nullptr; plain.hi = nullptr; plain.tag = nullptr;
-    if (lane == 0) work->huf.seg_count = reinterpret_cast<u32 (*)[256]>(seg_hist);
+    if (lane == 0) reinterpret_cast<EncWork*>(b.scratch + my_off)->huf.seg_count = reinterpret_cast<u32 (*)[256]>(seg_hist);
     __syncwarp();
     for (;;) {
         u32 unit = 0;
@@ -195,11 +185,32 @@ lizard_encode_units_kernel(EncodeBatch b, u32 smem_tables, u32 table_bytes, u32 
         if (unit >= b.n_units) break;
         progress_wait(b.progress, unit, lane);
         const u32 len = b.src_len[unit];
+        // The level's parameters, the warp's scratch base and its table base are derived per unit: kept for the whole
+        // kernel they took local-memory slots.  The two bases are then held in registers for the unit: left to itself
+        // the compiler re-derives them (a 64-bit multiply-add) in front of every access.
+        const LevelParams klp = level_params(b.level);
+        const bool tagged = enc_tagged(klp), tagged_plain = enc_tagged_plain(klp);
+        u8* my = b.scratch + my_off;
+        u8* tab = enc_smem + (size_t)wic * table_bytes;
+#if LZB_ENC_OPAQUE
+        asm volatile("" : "+l"(my));
+#endif
+#if LZB_ENC_OPAQUE >= 2
+        asm volatile("" : "+l"(tab));            // (generic instead of shared-space accesses to the packed table then)
+#endif
+        EncWork* work = reinterpret_cast<EncWork*>(my);
         // 17-bit packed entries need every position of the unit below 2^17
-        plain.tagged = (tagged_plain && len <= kBlockSize) ? 1u : 0u;      // 7 spare bits per entry when positions stay below 2^17
-        const HashTable& T = (packed_ok && len <= kBlockSize) ? packed : plain;
-        const int r = encode_unit<WarpLanes>(b.src_base + b.src_off[unit], len,
-                                             b.dst_base + b.dst_off[unit], b.dst_cap[unit], b.level, T, work);
+        HashTable T;
+        if (packed_ok && len <= kBlockSize) {
+            T.t32 = nullptr; T.lo = reinterpret_cast<u16*>(tab);
+            T.hi = reinterpret_cast<u32*>(tab + ((size_t)2 << klp.hashLog));
+            T.tag = tagged ? tab + hash_packed_bytes(klp.hashLog, false) : nullptr; T.tagged = 0;
+        } else {
+            T.t32 = reinterpret_cast<u32*>(my + sizeof(EncWork)); T.lo = nullptr; T.hi = nullptr; T.tag = nullptr;
+            T.tagged = (tagged_plain && len <= kBlockSize) ? 1u : 0u;      // 7 spare bits per entry when positions stay below 2^17
+        }
+        const int r = encode_unit_fam<WarpLanes, kFam>(b.src_base + b.src_off[unit], len,
+                                                       b.dst_base + b.dst_off[unit], b.dst_cap[unit], b.level, T, work);
         if (lane == 0) b.result[unit] = r;
         __syncwarp();
         if (b.pack.out) { pack_unit(b, unit, len, r, lane); __syncwarp(); pack_done(b, unit, lane); }
@@ -209,13 +220,24 @@ lizard_encode_units_kernel(EncodeBatch b, u32 smem_tables, u32 table_bytes, u32 
 
 inline size_t enc_align(size_t v) { return (v + 255) / 256 * 256; }
 
+typedef void (*EncodeKernel)(EncodeBatch, u32, u32, u32, size_t);
+inline EncodeKernel encode_kernel(int fam)
+{
+    switch (fam) {
+    case kEncFamFast:    return lizard_encode_units_kernel<kEncFamFast>;
+    case kEncFamFastBig: return lizard_encode_units_kernel<kEncFamFastBig>;
+    default:             return lizard_encode_units_kernel<kEncFamGeneric>;
+    }
+}
+
 inline int encode_context_init(EncodeConfig& c, int sm_count, int)
 {
     c.sm_count = sm_count;
     c.per_warp_small = enc_align(sizeof(EncWork) + kEncBigTableBytes);
     c.per_warp_big = c.per_warp_small;
-    if (cudaFuncSetAttribute(lizard_encode_units_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             227 * 1024) != cudaSuccess) return -1;
+    for (int f = 0; f < kEncFamilies; ++f)
+        if (cudaFuncSetAttribute(encode_kernel(f), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 227 * 1024) != cudaSuccess) return -1;
     c.max_warps = sm_count * kEncMaxWarpsPerSM;
     c.scratch_bytes = (size_t)c.max_warps * c.per_warp_small;
     return 0;
@@ -285,13 +307,15 @@ inline EncodeShape encode_shape_in_effect(const LevelParams& lp)
 
 inline cudaError_t encode_launch(const EncodeConfig& c, const EncodeBatch& b, cudaStream_t s, int* launches)
 {
-    const EncodeShape sh = encode_shape_in_effect(level_params(b.level));
+    const LevelParams lp = level_params(b.level);
+    const EncodeShape sh = encode_shape_in_effect(lp);
+    const EncodeKernel kern = encode_kernel(enc_family(lp));
     const size_t per_warp = c.per_warp_small;
     int per_sm = 0;
     // the occupancy query honours the kernel's current carve-out preference, which the previous launch (possibly of
     // another level) left behind: ask with the whole array available, then set what this launch uses
-    cudaFuncSetAttribute(lizard_encode_units_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lizard_encode_units_kernel, 32 * sh.warps, sh.smem);
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32 * sh.warps, sh.smem);
     if (e != cudaSuccess) return e;
     if (per_sm < 1) per_sm = 1;
     if (per_sm > sh.ctas_per_sm) per_sm = sh.ctas_per_sm;
@@ -303,10 +327,9 @@ inline cudaError_t encode_launch(const EncodeConfig& c, const EncodeBatch& b, cu
         const size_t total = 228 * 1024, use = (size_t)per_sm * (sh.smem + 1024);
         int pct = (int)((use * 100 + total - 1) / total);
         if (pct > 100) pct = 100;
-        cudaFuncSetAttribute(lizard_encode_units_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+        cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     }
-    lizard_encode_units_kernel<<<(unsigned)grid, 32 * sh.warps, sh.smem, s>>>(b, (u32)sh.smem_tables, (u32)sh.table_bytes,
-                                                                            (u32)sh.hist_bytes, per_warp);
+    kern<<<(unsigned)grid, 32 * sh.warps, sh.smem, s>>>(b, (u32)sh.smem_tables, (u32)sh.table_bytes, (u32)sh.hist_bytes, per_warp);
     *launches = 1;
     return cudaGetLastError();
 }

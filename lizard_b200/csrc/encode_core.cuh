@@ -265,6 +265,7 @@ struct HashTable {       // runtime descriptor handed to encode_unit
     u32  tagged;         // plain form: every position of the unit is below 2^17, bits 25..31 of an entry hold a tag
 };
 struct PlainTable {
+    static constexpr bool kOneBlock = false;    // any unit
     u32* t32; u32 tagged;
     LZ_HDM explicit PlainTable(const HashTable& d) : t32(d.t32), tagged(d.tagged) {}
     LZ_HDM u32 get(u32 h, u32) const { const u32 e = t32[h]; return tagged ? e & 0x1FFFFFFu : e; }
@@ -286,6 +287,7 @@ struct PlainTable {
     }
 };
 struct PackedTable {
+    static constexpr bool kOneBlock = true;     // units of one inner block only (positions below 2^17)
     u16* lo; u32* hi; u8* tag;
     LZ_HDM explicit PackedTable(const HashTable& d) : lo(d.lo), hi(d.hi), tag(d.tag) {}
     LZ_HDM u32 get(u32 h, u32 pos_hint) const
@@ -1220,13 +1222,37 @@ struct EncWork {                 // per-warp global scratch
     EncHufWork huf;
 };
 
-// Lizard_compress_extState with a clean table: returns compressed size or 0
-template <class W, class TT> LZ_HD int encode_unit_t(const u8* src, u32 src_size, u8* dst, u32 cap, int level,
-                                                    const TT T, EncWork* work)
+// ---- parser families -----------------------------------------------------------------------------------------
+// The encoder is compiled once per family so that a level only carries the code (and the register allocation) of the
+// parsers it can reach.  Fast: fastSmall / fast without an entropy stage (levels 10, 11); FastBig: fastBig without one
+// (level 20); Generic: every level, parser and Huffman stage picked at run time (hashChain, priceFast, 30/31/40).
+// The device launches the family's kernel instance; encode_unit() (host build, emulated warps) picks the same family
+// at run time, so both run the same per-family code.
+enum EncFamily : int { kEncFamFast = 0, kEncFamFastBig = 1, kEncFamGeneric = 2, kEncFamilies = 3 };
+LZ_HD int enc_family(const LevelParams& lp)
+{
+    if (lp.huffman) return kEncFamGeneric;
+    if (lp.parser == kParserFastSmall || lp.parser == kParserFast) return kEncFamFast;
+    if (lp.parser == kParserFastBig) return kEncFamFastBig;
+    return kEncFamGeneric;
+}
+
+// the fastSmall / fast / fastBig walk: window form on real and emulated warps, batch form on narrow lane policies
+template <class W, class TT, bool kBig> LZ_HD void parse_fast_any(const ParseCtx<TT>& pc, u32 b0, u32 b1, EncStreams& s)
+{
+    if (W::kLanes >= 4) parse_fast_win<W, TT, kBig>(pc, b0, b1, s);
+    else parse_fast_par<W, TT, kBig>(pc, b0, b1, s);
+}
+
+// Lizard_compress_extState with a clean table: returns compressed size or 0.  kFam fixes the parser (Fast, FastBig) and
+// compiles the entropy stage out of the families that never run it.
+template <class W, class TT, int kFam> LZ_HD int encode_unit_t(const u8* src, u32 src_size, u8* dst, u32 cap, int level,
+                                                              const TT T, EncWork* work)
 {
     const LevelParams lp = level_params(level);
     if (lp.parser == kParserUnsupported) return 0;
     if (src_size > kMaxInputSize) return 0;
+    if (TT::kOneBlock && src_size > kBlockSize) return 0;
     T.template clear<W>(lp.hashLog);
     const bool wr = W::lane() == 0;
     long op = 0;
@@ -1236,34 +1262,45 @@ template <class W, class TT> LZ_HD int encode_unit_t(const u8* src, u32 src_size
     op = 1;
     ParseCtx<TT> pc = { src, T, lp.hashLog, lp.windowLog };
     ChainState cs = { work->chain, (1u << (lp.chainLog ? lp.chainLog : 16)) - 1, 0, lp.searchNum, lp.searchLength };
+    const bool huffman = kFam == kEncFamGeneric && lp.huffman != 0;
+    const bool lizv1 = kFam == kEncFamFastBig || (kFam == kEncFamGeneric && lp.lizv1 != 0);
     u32 pos = 0;
     while (pos < src_size) {
         const u32 part = src_size - pos < kBlockSize ? src_size - pos : kBlockSize;
         EncStreams s;
         s.rec = work->seq; s.nseq = 0;
         s.nl = s.nf = s.n16 = s.n24 = 0; s.tail_anchor = pos; s.tail_len = 0;
-        if (lp.parser == kParserHashChain) parse_hash_chain<W, TT>(pc, pos, pos + part, s, cs);
+        if (kFam == kEncFamFast) parse_fast_any<W, TT, false>(pc, pos, pos + part, s);
+        else if (kFam == kEncFamFastBig) parse_fast_any<W, TT, true>(pc, pos, pos + part, s);
+        else if (lp.parser == kParserHashChain) parse_hash_chain<W, TT>(pc, pos, pos + part, s, cs);
         else if (lp.parser == kParserPriceFast) parse_price_fast_par<W, TT>(pc, pos, pos + part, s, lp.minMatchLongOff);
-        else if (lp.parser == kParserFastBig) {
-            if (W::kLanes >= 4) parse_fast_win<W, TT, true>(pc, pos, pos + part, s);
-            else parse_fast_par<W, TT, true>(pc, pos, pos + part, s);
-        }
-        else if (W::kLanes >= 4) parse_fast_win<W, TT>(pc, pos, pos + part, s);
-        else parse_fast_par<W, TT>(pc, pos, pos + part, s);
+        else if (lp.parser == kParserFastBig) parse_fast_any<W, TT, true>(pc, pos, pos + part, s);
+        else parse_fast_any<W, TT, false>(pc, pos, pos + part, s);
         W::sync();
-        if (write_block<W>(s, src, src + pos, part, dst, op, oend, lp.huffman != 0, lp.lizv1 != 0,
+        if (write_block<W>(s, src, src + pos, part, dst, op, oend, huffman, lizv1,
                            work->lits, work->flags, &work->huf)) return 0;
         W::sync();
+        if (TT::kOneBlock) break;   // a packed table serves one inner block: the loop state is dead while it is written
         pos += part;
     }
     return (int)op;
 }
-// the packed form only holds positions of a single inner block
+// one family; the packed form only holds positions of a single inner block
+template <class W, int kFam> LZ_HD int encode_unit_fam(const u8* src, u32 src_size, u8* dst, u32 cap, int level,
+                                                      const HashTable& T, EncWork* work)
+{
+    if (T.t32) return encode_unit_t<W, PlainTable, kFam>(src, src_size, dst, cap, level, PlainTable(T), work);
+    return encode_unit_t<W, PackedTable, kFam>(src, src_size, dst, cap, level, PackedTable(T), work);
+}
+// the level's family picked at run time
 template <class W> LZ_HD int encode_unit(const u8* src, u32 src_size, u8* dst, u32 cap, int level,
                                         const HashTable& T, EncWork* work)
 {
-    if (T.t32) return encode_unit_t<W, PlainTable>(src, src_size, dst, cap, level, PlainTable(T), work);
-    return encode_unit_t<W, PackedTable>(src, src_size, dst, cap, level, PackedTable(T), work);
+    switch (enc_family(level_params(level))) {
+    case kEncFamFast:    return encode_unit_fam<W, kEncFamFast>(src, src_size, dst, cap, level, T, work);
+    case kEncFamFastBig: return encode_unit_fam<W, kEncFamFastBig>(src, src_size, dst, cap, level, T, work);
+    default:             return encode_unit_fam<W, kEncFamGeneric>(src, src_size, dst, cap, level, T, work);
+    }
 }
 
 }  // namespace lzb
