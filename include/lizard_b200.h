@@ -12,6 +12,7 @@
  *        lib/lizard_compress.h:146   Lizard_sizeofState       lib/lizard_compress.c:311-323
  *        lib/lizard_compress.h:147   Lizard_compress_extState lib/lizard_compress.c:583-593
  *        lib/lizard_decompress.h:73  Lizard_decompress_safe   lib/lizard_decompress.c:267-270
+ *        lib/lizard_decompress.h:89  Lizard_decompress_safe_partial lib/lizard_decompress.c:272-275
  *      Compression output is byte-identical to the reference built with -DLIZARD_RESET_MEM
  *      (hash table empty at the start of every call), for the levels whose parsers are implemented on
  *      the GPU: 10, 11, 30, 31 (fastSmall / fast), 13-17, 34-38 (hashChain), 20, 40 (fastBig) and 21, 22, 41, 42 (priceFast).
@@ -73,6 +74,14 @@ int Lizard_compress_extState(void* state, const char* src, char* dst, int srcSiz
  * following block past dst + maxDecompressedSize and reports success.  This library never writes outside
  * [dst, dst + maxDecompressedSize): it is the safer of the two. */
 int Lizard_decompress_safe(const char* src, char* dst, int compressedSize, int maxDecompressedSize);
+/* decodes until at least targetOutputSize bytes are out, then stops; returns the decoded size (which may exceed the target),
+ * or a negative error, exactly as the reference (lib/lizard_decompress.c:115-264 with partialDecoding), quirks included:
+ * each inner block's token loop measures the target from the START OF THAT BLOCK (so a target inside the second block of a
+ * unit decodes that block whole), the fastLZ4 codewords stop after a token's literals or its match (a block that stops after
+ * its last match does not copy its last literals), the LIZv1 codewords stop in front of a token.  Nothing behind the
+ * stopping point is read: damage there is not reported.  Bytes behind the returned size are unspecified.  With
+ * targetOutputSize >= the decoded size this is Lizard_decompress_safe. */
+int Lizard_decompress_safe_partial(const char* source, char* dest, int compressedSize, int targetOutputSize, int maxDecompressedSize);
 
 /* ---------------------------------------------------------------------------------------------
  * (1a) the rest of the reference's export list (lib/dll/liblizard.def:3-19), so that its own callers link:
@@ -81,8 +90,9 @@ int Lizard_decompress_safe(const char* src, char* dst, int compressedSize, int m
  *      Lizard_compress_extState.  The streaming / dictionary family (linked blocks, cross-call windows;
  *      lib/lizard_compress.h:178-198, lib/lizard_decompress.h:89-145) is OUT OF SCOPE and fails with the reference's
  *      failure values: 0 from Lizard_loadDict / Lizard_saveDict / Lizard_compress_continue, -1 from
- *      Lizard_decompress_safe_continue / _partial; Lizard_decompress_safe_usingDict is Lizard_decompress_safe when
+ *      Lizard_decompress_safe_continue; Lizard_decompress_safe_usingDict is Lizard_decompress_safe when
  *      dictSize == 0 (lib/lizard_decompress.c:353-355) and -1 with a dictionary.  No CPU code path behind any of them.
+ *      (Lizard_decompress_safe_partial is not part of that family: it is implemented, see (1).)
  * ------------------------------------------------------------------------------------------- */
 typedef struct Lizard_stream_s Lizard_stream_t;                 /* lib/lizard_compress.h:72 */
 typedef struct Lizard_streamDecode_s Lizard_streamDecode_t;     /* lib/lizard_decompress.h:100 */
@@ -92,7 +102,6 @@ Lizard_stream_t* Lizard_resetStream(Lizard_stream_t* streamPtr, int compressionL
 int Lizard_loadDict(Lizard_stream_t* streamPtr, const char* dictionary, int dictSize);
 int Lizard_saveDict(Lizard_stream_t* streamPtr, char* safeBuffer, int dictSize);
 int Lizard_compress_continue(Lizard_stream_t* streamPtr, const char* src, char* dst, int srcSize, int maxDstSize);
-int Lizard_decompress_safe_partial(const char* source, char* dest, int compressedSize, int targetOutputSize, int maxDecompressedSize);
 Lizard_streamDecode_t* Lizard_createStreamDecode(void);
 int Lizard_freeStreamDecode(Lizard_streamDecode_t* streamPtr);
 int Lizard_setStreamDecode(Lizard_streamDecode_t* streamPtr, const char* dictionary, int dictSize);
@@ -173,6 +182,12 @@ int LizardB200_compress_batch(const void* const* src, const int* srcSize,
 /* result[i] as Lizard_decompress_safe */
 int LizardB200_decompress_batch(const void* const* src, const int* compressedSize,
                                 void* const* dst, const int* dstCapacity, int* result, int nUnits);
+/* result[i] as Lizard_decompress_safe_partial(src[i], dst[i], compressedSize[i], targetOutputSize[i], dstCapacity[i]):
+ * a warp stops at its unit's target and takes the next unit.  One launch of the partial-decode kernel, whatever
+ * LizardB200_setDecodeVariant says (it never runs the pre-passes, which expand or parse whole streams). */
+int LizardB200_decompress_partial_batch(const void* const* src, const int* compressedSize,
+                                        void* const* dst, const int* dstCapacity, const int* targetOutputSize,
+                                        int* result, int nUnits);
 
 /* Contiguous host buffers, units described by offset/size arrays (what a frame or a file splitter has).
  * dstStride: unit i is written at dst + i*dstStride with capacity dstCapacityEach. */
@@ -193,6 +208,10 @@ int LizardB200_decompress_blocks(const void* src, size_t srcStride, const int* c
 int LizardB200_decompress_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
                                  void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
                                  int* dResult, unsigned nUnits, void* cudaStream);
+/* partial decode of every unit, dTarget[i] = its targetOutputSize (device memory); same workspace and stream rules */
+int LizardB200_decompress_partial_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
+                                         void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
+                                         const int* dTarget, int* dResult, unsigned nUnits, void* cudaStream);
 int LizardB200_compress_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
                                void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
                                int* dResult, unsigned nUnits, int compressionLevel, void* cudaStream);

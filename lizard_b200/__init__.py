@@ -42,8 +42,11 @@ def lib():
         L.LizardB200_launchCount.restype = ctypes.c_ulonglong
         L.LizardB200_compress_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int, ctypes.c_int]
         L.LizardB200_decompress_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int]
+        L.Lizard_decompress_safe_partial.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+        L.LizardB200_decompress_partial_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, c_int_p, ctypes.c_int]
         dev_args = [ctypes.c_void_p] * 7 + [ctypes.c_uint]
         L.LizardB200_decompress_device.argtypes = dev_args + [ctypes.c_void_p]
+        L.LizardB200_decompress_partial_device.argtypes = [ctypes.c_void_p] * 8 + [ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_compress_device.argtypes = dev_args + [ctypes.c_int, ctypes.c_void_p]
         L.LizardB200_gather_device.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_compress_blocks.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p,
@@ -80,7 +83,16 @@ def decompress(src: bytes, max_size: int):
     return r, (dst.raw[:r] if r > 0 else b"")
 
 
-def _batch(fn, units, caps, extra):
+def decompress_partial(src: bytes, target: int, max_size: int):
+    """Lizard_decompress_safe_partial on host bytes -> (return code, bytes).  Decoding stops once `target` bytes are out;
+    the return code may exceed the target (the reference's stopping rules, include/lizard_b200.h)."""
+    L = lib()
+    dst = ctypes.create_string_buffer(max(max_size, 1))
+    r = L.Lizard_decompress_safe_partial(src, dst, len(src), target, max_size)
+    return r, (dst.raw[:r] if r > 0 else b"")
+
+
+def _batch(fn, units, caps, extra, targets=None):
     n = len(units)
     srcs = (ctypes.c_void_p * n)()
     sizes = (ctypes.c_int * n)()
@@ -97,7 +109,10 @@ def _batch(fn, units, caps, extra):
         outs.append(o)
         dsts[i] = ctypes.cast(o, ctypes.c_void_p)
         dcaps[i] = caps[i]
-    st = fn(srcs, sizes, dsts, dcaps, res, n, *extra)
+    if targets is None:
+        st = fn(srcs, sizes, dsts, dcaps, res, n, *extra)
+    else:
+        st = fn(srcs, sizes, dsts, dcaps, (ctypes.c_int * n)(*targets), res, n, *extra)
     _check(st, "batch call")
     return [(res[i], outs[i].raw[:res[i]] if res[i] > 0 else b"") for i in range(n)]
 
@@ -112,6 +127,14 @@ def compress_batch(units, level, caps=None):
 def decompress_batch(units, caps):
     """LizardB200_decompress_batch: list of compressed bytes -> list of (result, bytes)."""
     return _batch(lib().LizardB200_decompress_batch, units, caps, ())
+
+
+def decompress_partial_batch(units, targets, caps):
+    """LizardB200_decompress_partial_batch: list of compressed bytes, per-unit targetOutputSize and capacity -> list of
+    (result, bytes), each as decompress_partial."""
+    if len(targets) != len(units):
+        raise ValueError("one target per unit")
+    return _batch(lib().LizardB200_decompress_partial_batch, units, caps, (), targets)
 
 
 def _load_dg():

@@ -32,10 +32,9 @@ namespace {
 constexpr int kDecWarps = LZB_DEC_WARPS;     // warps per CTA in the decode kernel (x 4 CTAs per SM)
 constexpr int kMaxDevices = 16;
 
-// V = schedule of the token loops, two bits: 1 = pooled copy sweeps, 2 = compact length-extension chain (default 3 = both;
-// LIZARDB200_DEC_VARIANT=0..3 or LizardB200_setDecodeVariant select the others for A/B runs)
-template <int V> __global__ void __launch_bounds__(kDecWarps * 32, 4)
-lizard_decode_units_kernel(DecodeBatch b)
+// Body of the first-generation decode kernels: a persistent set of warps, one unit per warp at a time.
+// kPartial: Lizard_decompress_safe_partial with the unit's b.target instead of Lizard_decompress_safe.
+template <int V, bool kPartial> __device__ __forceinline__ void decode_units(const DecodeBatch& b)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const u32 warp = threadIdx.x >> 5, lane = WarpLanes::lane();
@@ -55,14 +54,34 @@ lizard_decode_units_kernel(DecodeBatch b)
         unit = __shfl_sync(LZB_FULL, unit, 0);
         if (unit >= b.n_units) break;
         progress_wait(b.progress, unit, lane);
-        const int r = decode_unit<WarpLanes, V>(b.src_base + b.src_off[unit], b.src_len[unit],
-                                                b.dst_base + b.dst_off[unit], b.dst_cap[unit], scratch, sh,
-                                                b.pre ? b.pre + unit : nullptr, b.arena,
-                                                b.seq ? b.seq + unit : nullptr, b.recs);
+        int r;
+        if constexpr (kPartial) r = decode_unit<WarpLanes, V, true>(b.src_base + b.src_off[unit], b.src_len[unit],
+                                                          b.dst_base + b.dst_off[unit], b.dst_cap[unit], scratch, sh,
+                                                          nullptr, nullptr, nullptr, nullptr, b.target[unit]);
+        else r = decode_unit<WarpLanes, V>(b.src_base + b.src_off[unit], b.src_len[unit],
+                                           b.dst_base + b.dst_off[unit], b.dst_cap[unit], scratch, sh,
+                                           b.pre ? b.pre + unit : nullptr, b.arena,
+                                           b.seq ? b.seq + unit : nullptr, b.recs);
         if (lane == 0) b.result[unit] = r;
         __syncwarp();
         progress_done(b.progress, unit, lane);
     }
+}
+
+// V = schedule of the token loops, two bits: 1 = pooled copy sweeps, 2 = compact length-extension chain (default 3 = both;
+// LIZARDB200_DEC_VARIANT=0..3 or LizardB200_setDecodeVariant select the others for A/B runs)
+template <int V> __global__ void __launch_bounds__(kDecWarps * 32, 4)
+lizard_decode_units_kernel(DecodeBatch b)
+{
+    decode_units<V, false>(b);
+}
+
+// Partial decode (LizardB200_decompress_partial_*): a kernel of its own, so that the full decode above keeps its code.  It runs
+// the default schedule and never the pre-passes, which expand or parse whole streams that a partial unit may never reach.
+constexpr int kDecPartialSchedule = 3;
+__global__ void __launch_bounds__(kDecWarps * 32, 4) lizard_decode_partial_units_kernel(DecodeBatch b)
+{
+    decode_units<kDecPartialSchedule, true>(b);
 }
 
 // Variable-length segments to their places in another arena (segment i: src_off[i], len[i] -> dst_off[i]): what the frame
@@ -170,6 +189,7 @@ struct Context {
     bool ready = false, failed = false;
     int device = 0, sm_count = 0;
     cudaStream_t stream = nullptr, s_in = nullptr, s_out = nullptr;   // compute / H2D / D2H
+    int decp_grid = 0;                        // grid of the partial-decode kernel
     int dec_grid = 0, dec_variant = 7;        // bits 0-1: schedule of the token loops, bit 2: Huffman pre-pass, bit 3: token pre-pass,
                                               // bit 4: second-generation kernel (parser + copier warp per unit)
     int dec2_grid = 0, dec2_stages = 4;
@@ -271,6 +291,17 @@ int ensure_context(Context& c, int device)
     for (int v = 0; v < 4; ++v)
         cudaFuncSetAttribute(decode_kernel(v), cudaFuncAttributePreferredSharedMemoryCarveout,
                              carveout((size_t)per_sm * (dec_smem + 1024), "LIZARDB200_DEC_CARVEOUT"));
+    {   // partial decode: same launch shape and scratch as the full decode, its own kernel
+        int pp = 0;
+        e = cudaFuncSetAttribute(lizard_decode_partial_units_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec_smem);
+        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pp, lizard_decode_partial_units_kernel, kDecWarps * 32, dec_smem);
+        if (e != cudaSuccess) { c.failed = true; fail("cudaFuncSetAttribute(partial decode)", e); return LIZARDB200_ERR_CUDA; }
+        if (pp < 1) pp = 1;
+        if (pp > per_sm) pp = per_sm;                 // the scratch below is sized for dec_grid
+        c.decp_grid = c.sm_count * pp;
+        cudaFuncSetAttribute(lizard_decode_partial_units_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                             carveout((size_t)pp * (dec_smem + 1024), "LIZARDB200_DEC_CARVEOUT"));
+    }
     {   // second generation: CTAs of two warps, static shared memory; as many per SM as fit (LIZARDB200_DEC2_CTAS_PER_SM caps it)
         if (const char* v = getenv("LIZARDB200_DEC2_STAGES")) c.dec2_stages = atoi(v) >= 8 ? 8 : 4;
         cudaFuncAttributes fa;
@@ -410,7 +441,7 @@ int launch_decode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* d
     b.result = dResult; b.n_units = n;
     b.scratch = (u8*)c.dec_scratch.p;
     b.counter = next_counter(c, s);
-    b.pre = nullptr; b.arena = nullptr; b.seq = nullptr; b.recs = nullptr;
+    b.pre = nullptr; b.arena = nullptr; b.seq = nullptr; b.recs = nullptr; b.target = nullptr;
     if ((c.dec_variant & 4) && pg == nullptr && n >= kPrepassMinUnits) {
         int st = launch_prepass(c, b, s);
         if (st != LIZARDB200_OK) return st;
@@ -430,6 +461,30 @@ int launch_decode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* d
     int grid = (int)((warps_needed + kDecWarps - 1) / kDecWarps);
     if (grid > c.dec_grid) grid = c.dec_grid;
     decode_kernel(c.dec_variant)<<<grid, kDecWarps * 32, sizeof(DecWarpShared) * kDecWarps, s>>>(b);
+    g_launches++;
+    CU_OK(cudaGetLastError());
+    return LIZARDB200_OK;
+}
+
+// Lizard_decompress_safe_partial for every unit, dTarget[i] = unit i's targetOutputSize: one launch of the partial kernel,
+// whatever the decode variant (no pre-pass, no second generation).
+int launch_decode_partial(Context& c, const void* dSrc, const u64* dSrcOff, const u32* dSrcLen,
+                          void* dDst, const u64* dDstOff, const u32* dDstCap, const int* dTarget, int* dResult, u32 n,
+                          cudaStream_t s)
+{
+    if (n == 0) return LIZARDB200_OK;
+    workspace_acquire(c, s);
+    struct Release { Context& c; cudaStream_t s; ~Release() { workspace_release(c, s); } } release_on_exit{c, s};
+    DecodeBatch b;
+    memset(&b, 0, sizeof b);
+    b.src_base = (const u8*)dSrc; b.src_off = dSrcOff; b.src_len = dSrcLen;
+    b.dst_base = (u8*)dDst; b.dst_off = dDstOff; b.dst_cap = dDstCap;
+    b.result = dResult; b.n_units = n; b.target = dTarget;
+    b.scratch = (u8*)c.dec_scratch.p;
+    b.counter = next_counter(c, s);
+    int grid = (int)((n + kDecWarps - 1) / kDecWarps);
+    if (grid > c.decp_grid) grid = c.decp_grid;
+    lizard_decode_partial_units_kernel<<<grid, kDecWarps * 32, sizeof(DecWarpShared) * kDecWarps, s>>>(b);
     g_launches++;
     CU_OK(cudaGetLastError());
     return LIZARDB200_OK;
@@ -462,9 +517,10 @@ int launch_encode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* d
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // Shared body of the host-pointer batch calls: stage inputs + tables, run, fetch results + outputs.
+// `target` (decode only): per-unit targetOutputSize of a partial decode, null for a full one.
 template <bool kCompress>
 int run_host_batch(const void* const* src, const int* srcSize, void* const* dst, const int* dstCap,
-                   int* result, int n, int level)
+                   int* result, int n, int level, const int* target = nullptr)
 {
     if (n < 0 || (n > 0 && (!src || !srcSize || !dst || !dstCap || !result))) return LIZARDB200_ERR_ARGUMENT;
     if (n == 0) return LIZARDB200_OK;
@@ -485,7 +541,7 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
         in_off[i] = in_total;   in_total += align_up((size_t)srcSize[i] + 16, 16);
         out_off[i] = out_total; out_total += align_up((size_t)dstCap[i] + 32, 16);
     }
-    const size_t tab_bytes = (size_t)n * (8 + 4 + 8 + 4 + 4);
+    const size_t tab_bytes = (size_t)n * (8 + 4 + 8 + 4 + (target ? 4 : 0) + 4);
     CU_OK(c.pin_in.reserve(in_total));
     CU_OK(c.pin_tab.reserve(tab_bytes));
     CU_OK(c.d_in.reserve(in_total));
@@ -498,11 +554,13 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
     u64* t_out_off = t_in_off + n;
     u32* t_in_len = (u32*)(t_out_off + n);
     u32* t_out_cap = t_in_len + n;
-    int* t_res = (int*)(t_out_cap + n);
+    int* t_target = (int*)(t_out_cap + n);
+    int* t_res = t_target + (target ? n : 0);
     for (int i = 0; i < n; ++i) {
         memcpy((u8*)c.pin_in.p + in_off[i], src[i], (size_t)srcSize[i]);
         t_in_off[i] = in_off[i]; t_out_off[i] = out_off[i];
         t_in_len[i] = (u32)srcSize[i]; t_out_cap[i] = (u32)dstCap[i];
+        if (target) t_target[i] = target[i];
     }
     u8* dtab = (u8*)c.d_tab.p;
     cudaStream_t s = c.stream;
@@ -512,8 +570,10 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
     const u64* d_out_off = d_in_off + n;
     const u32* d_in_len = (const u32*)(d_out_off + n);
     const u32* d_out_cap = d_in_len + n;
-    int* d_res = (int*)(d_out_cap + n);
+    const int* d_target = (const int*)(d_out_cap + n);
+    int* d_res = (int*)d_target + (target ? n : 0);
     if (kCompress) st = launch_encode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, level, s);
+    else if (target) st = launch_decode_partial(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_target, d_res, (u32)n, s);
     else           st = launch_decode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, s);
     if (st != LIZARDB200_OK) return st;
     CU_OK(cudaMemcpyAsync(t_res, d_res, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
@@ -603,6 +663,18 @@ int LizardB200_decompress_device(const void* dSrc, const uint64_t* dSrcOff, cons
     if (st != LIZARDB200_OK) return st;
     return launch_decode(c, dSrc, (const u64*)dSrcOff, dSrcLen, dDst, (const u64*)dDstOff, dDstCap, dResult, nUnits, (cudaStream_t)stream);
 }
+int LizardB200_decompress_partial_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
+                                         void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
+                                         const int* dTarget, int* dResult, unsigned nUnits, void* stream)
+{
+    if (nUnits > 0 && !dTarget) return LIZARDB200_ERR_ARGUMENT;
+    Context& c = g_ctx[g_device];
+    std::lock_guard<std::mutex> lock(c.mu);
+    int st = ensure_context(c, g_device);
+    if (st != LIZARDB200_OK) return st;
+    return launch_decode_partial(c, dSrc, (const u64*)dSrcOff, dSrcLen, dDst, (const u64*)dDstOff, dDstCap, dTarget, dResult, nUnits,
+                                 (cudaStream_t)stream);
+}
 int LizardB200_compress_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
                                void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
                                int* dResult, unsigned nUnits, int level, void* stream)
@@ -635,6 +707,12 @@ int LizardB200_decompress_batch(const void* const* src, const int* cSize, void* 
                                 int* result, int n)
 {
     return run_host_batch<false>(src, cSize, dst, dstCap, result, n, 0);
+}
+int LizardB200_decompress_partial_batch(const void* const* src, const int* cSize, void* const* dst, const int* dstCap,
+                                        const int* targetOutputSize, int* result, int n)
+{
+    if (n > 0 && !targetOutputSize) return LIZARDB200_ERR_ARGUMENT;
+    return run_host_batch<false>(src, cSize, dst, dstCap, result, n, 0, targetOutputSize);
 }
 int LizardB200_compress_batch(const void* const* src, const int* srcSize, void* const* dst, const int* dstCap,
                               int* result, int n, int level)
@@ -791,10 +869,14 @@ int Lizard_setStreamDecode(Lizard_streamDecode_t* p, const char* dict, int dictS
     return 1;
 }
 int Lizard_decompress_safe_continue(Lizard_streamDecode_t*, const char*, char*, int, int) { g_last_error = kNoStreaming; return -1; }
-int Lizard_decompress_safe_partial(const char*, char*, int, int, int)
+int Lizard_decompress_safe_partial(const char* src, char* dst, int compressedSize, int targetOutputSize, int maxDecompressedSize)
 {
-    g_last_error = "Lizard_decompress_safe_partial is not implemented on the GPU path";
-    return -1;
+    // same argument handling as Lizard_decompress_safe (lib/lizard_decompress.c:139, 272-275)
+    if (compressedSize < 1) return 0;
+    if (maxDecompressedSize < 0) return -1;
+    const void* s = src; void* d = dst; int r = -1;
+    int st = LizardB200_decompress_partial_batch(&s, &compressedSize, &d, &maxDecompressedSize, &targetOutputSize, &r, 1);
+    return st == LIZARDB200_OK ? r : st;
 }
 int Lizard_decompress_safe_usingDict(const char* src, char* dst, int compressedSize, int maxDecompressedSize,
                                      const char* dictStart, int dictSize)

@@ -94,6 +94,7 @@ struct DecodeBatch {
     const u8*  arena;       // the pre-pass's expansion arena
     const UnitSeq* seq;     // [n] blocks parsed by the token pre-pass, or null
     const PoolRun* recs;    // its sequence records
+    const int* target;      // [n] targetOutputSize of a partial decode (lizard_decode_partial_units_kernel), null for a full one
 };
 
 enum : u32 { kDecStreamScratch = kBlockSize + 64, kDecBigTableBytes = 2u << kHufTableLogMax,
@@ -522,7 +523,8 @@ struct TokCursor { u32 fp; long lp; long op; u32 p16, p24; u32 last_off; };
 
 // ---- serial path: the reference's loop, one token at a time (all lanes in lock step) ------------------
 // Returns 0 to continue, or the (negative) error code.  Runs at most `count` tokens.
-template <class W> LZ_HD int lz4_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count)
+// kPartial (Lizard_decompress_safe_partial): returns 1 when the reference's loop stops at `oexit`, with c.op where it stopped.
+template <class W, bool kPartial = false> LZ_HD int lz4_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count, long oexit = 0)
 {
     const long nl = (long)s.nlits;
     for (u32 t = 0; t < count && c.fp < s.nflags; ++t) {
@@ -535,6 +537,7 @@ template <class W> LZ_HD int lz4_serial(const Streams& s, u8* dst, long oend, To
         if (c.op + len > oend - 16 || c.lp + len > nl - 18) return -(int)c.fp - 1;
         lanes_copy<W>(dst + c.op, s.lits + c.lp, len);
         c.op += len; c.lp += len;
+        if (kPartial && c.op >= oexit) { W::sync(); return 1; }    // lizard_decompress_lz4.h:82, before the offset is read
         const u32 off = rd_le16(s.lits + c.lp); c.lp += 2;
         if ((long)off > c.op) return -(int)c.fp - 1;               // match < lowLimit
         u32 ml = tok >> 4;
@@ -548,14 +551,16 @@ template <class W> LZ_HD int lz4_serial(const Streams& s, u8* dst, long oend, To
         lanes_match<W>(dst, c.op, off, ml);
         W::sync();
         c.op += ml;
+        if (kPartial && c.op >= oexit) return 1;                    // :144, the block's last literals are not copied
     }
     return 0;
 }
 
-template <class W> LZ_HD int lizv1_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count)
+template <class W, bool kPartial = false> LZ_HD int lizv1_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count, long oexit = 0)
 {
     const long nl = (long)s.nlits;
     for (u32 t = 0; t < count && c.fp < s.nflags; ++t) {
+        if (kPartial && c.op >= oexit) return 1;                    // lizard_decompress_liz.h:55, before the flags byte is read
         const u32 tok = s.flags[c.fp++];
         u32 ml;
         if (tok >= 32) {
@@ -1074,7 +1079,10 @@ template <class W> LZ_HD bool ext_chain_win(const u8* lits, u32 nl, u32 lp, u32 
 
 // fastLZ4 codewords (lib/lizard_decompress_lz4.h:7-163).  `op0` is the offset inside the unit's output,
 // `oend` the unit's capacity; matches may reach back to offset 0 of the unit.
-template <class W, int V> LZ_HD int decode_tokens_lz4(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh)
+// kPartial: the loop of Lizard_decompress_safe_partial, which returns as soon as the output reaches `oexit` (= op0 + the
+// target: the reference measures the target from the start of the inner block), after a token's literals or after its match.
+template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lz4(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh,
+                                                                   long oexit)
 {
     const long nl = (long)s.nlits, oend = (long)oend_u;
     const u32 NL = W::lanes(), lane = W::lane();
@@ -1185,10 +1193,30 @@ template <class W, int V> LZ_HD int decode_tokens_lz4(const Streams& s, u8* dst,
             u32 tot_out = 0;
             const u32 O = W::excl_scan((act && !bad) ? lit_len + ml : 0, &tot_out);
             const long opos = c.op + (long)O;
+            bool xl = false, xm = false;                                // kPartial: the reference stops after this token's literals / match
             if (act && !bad) {
                 if (opos + (long)lit_len > oend - 16) bad = true;
+                else if (kPartial && opos + (long)lit_len >= oexit) xl = true;
                 else if ((long)off > opos + (long)lit_len) bad = true;
                 else if (opos + (long)lit_len + (long)ml > oend - 16) bad = true;
+                else if (kPartial && opos + (long)lit_len + (long)ml >= oexit) xm = true;
+            }
+            if (kPartial) {
+                // The first lane that reaches oexit ends the block.  Its position is exact when no earlier lane failed a check
+                // (a failed lane adds nothing to the scan): then the batch shrinks to the tokens up to it, and failures behind
+                // it are never looked at.  Otherwise the serial path below meets the earlier error, or the exit, itself.
+                const u32 xs = W::ballot(xl || xm);
+                if (xs != 0) {
+                    const u32 e = ctz32(xs);
+                    if ((W::ballot(bad) & ((2u << e) - 1u)) == 0) {
+                        if (xl) ml = 0;                                 // lane e: literals only; the lanes behind it do not run
+                        const u32 end = W::shfl(O + lit_len + ml, e);
+                        if ((V & 1) == 0) run_batch_copies<W>(dst, s.lits, e + 1, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                        else run_batch_copies_pool<W>(dst, s.lits, e + 1, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                        W::sync();
+                        return (int)(c.op + (long)end - (long)op0);
+                    }
+                }
             }
             if (W::ballot(bad) == 0) {
                 LZB_COUNT_FAST(W::lane() == 0 ? nb : 0);
@@ -1203,8 +1231,9 @@ template <class W, int V> LZ_HD int decode_tokens_lz4(const Streams& s, u8* dst,
             }
         }
         LZB_COUNT_SLOW(W::lane() == 0 ? nb : 0);
-        const int e = lz4_serial<W>(s, dst, oend, c, nb);
+        const int e = lz4_serial<W, kPartial>(s, dst, oend, c, nb, oexit);
         if (e < 0) return e;
+        if (kPartial && e > 0) return (int)(c.op - (long)op0);
     }
     const long rest = nl - c.lp;
     if (rest < 0 || c.op + rest > oend) return -(int)c.fp - 1;
@@ -1216,7 +1245,10 @@ template <class W, int V> LZ_HD int decode_tokens_lz4(const Streams& s, u8* dst,
 }
 
 // LIZv1 codewords (lib/lizard_decompress_liz.h:14-220)
-template <class W, int V> LZ_HD int decode_tokens_lizv1(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh)
+// kPartial: the loop of Lizard_decompress_safe_partial, which returns in front of the first token that starts at or behind
+// `oexit` (op0 + the target); once the flags run out, the block's last literals are copied whatever the target.
+template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lizv1(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh,
+                                                                     long oexit)
 {
     const long nl = (long)s.nlits, oend = (long)oend_u;
     const u32 NL = W::lanes(), lane = W::lane();
@@ -1331,6 +1363,24 @@ template <class W, int V> LZ_HD int decode_tokens_lizv1(const Streams& s, u8* ds
                 else if ((long)off > opos + (long)lit_len) bad = true;
                 else if (opos + (long)lit_len + (long)ml > oend - 16) bad = true;
             }
+            if (kPartial) {
+                // The first lane that starts at or behind oexit ends the block before its token is read.  Its position is exact
+                // when no earlier lane failed a check: then only the lanes in front of it run.  Otherwise the serial path below
+                // meets the earlier error, or the exit, itself.
+                const u32 xs = W::ballot(act && opos >= oexit);
+                if (xs != 0) {
+                    const u32 e = ctz32(xs);
+                    if ((W::ballot(bad) & ((1u << e) - 1u)) == 0) {
+                        const u32 end = W::shfl(O, e);
+                        if (e > 0) {
+                            if ((V & 1) == 0) run_batch_copies<W>(dst, s.lits, e, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                            else run_batch_copies_pool<W>(dst, s.lits, e, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                            W::sync();
+                        }
+                        return (int)(c.op + (long)end - (long)op0);
+                    }
+                }
+            }
             if (W::ballot(bad) == 0) {
                 LZB_COUNT_FAST(W::lane() == 0 ? nb : 0);
                 if (LZB_DEC_LIT_PF_NEXT) { const long nx = c.lp + (long)tot_adv + (long)tot_ext + 128 * (long)lane; if (lane < LZB_DEC_LIT_PF_LINES && nx < nl) W::prefetch(s.lits + nx); }
@@ -1343,8 +1393,9 @@ template <class W, int V> LZ_HD int decode_tokens_lizv1(const Streams& s, u8* ds
             }
         }
         LZB_COUNT_SLOW(W::lane() == 0 ? nb : 0);
-        const int e = lizv1_serial<W>(s, dst, oend, c, nb);
+        const int e = lizv1_serial<W, kPartial>(s, dst, oend, c, nb, oexit);
         if (e < 0) return e;
+        if (kPartial && e > 0) return (int)(c.op - (long)op0);
     }
     const long rest = nl - c.lp;
     if (rest < 0 || c.op + rest > oend) return -(int)c.fp - 1;
@@ -1404,9 +1455,13 @@ template <class W> LZ_HD int read_stream(bool huff, const u8* src, long csize, l
 }
 
 // Lizard_decompress_safe for one unit; every lane returns the same value.
-template <class W, int V> LZ_HD int decode_unit(const u8* src, u32 csize_u, u8* dst, u32 cap, u8* scratch, DecWarpShared* sh,
-                                                const UnitPre* up = nullptr, const u8* arena = nullptr,
-                                                const UnitSeq* us = nullptr, const PoolRun* recs = nullptr)
+// kPartial: Lizard_decompress_safe_partial with targetOutputSize = `target` (lib/lizard_decompress.c:272-275).  The unit stops
+// after the inner block that brings its output to `target` or beyond (:175 for a raw block, :249), and each block's token
+// loop stops at its own start + `target`.  Nothing behind the stopping point is read.  Partial units never use the pre-passes.
+template <class W, int V, bool kPartial = false>
+LZ_HD int decode_unit(const u8* src, u32 csize_u, u8* dst, u32 cap, u8* scratch, DecWarpShared* sh,
+                      const UnitPre* up = nullptr, const u8* arena = nullptr,
+                      const UnitSeq* us = nullptr, const PoolRun* recs = nullptr, int target = 0)
 {
     const long csize = (long)csize_u;
     if (csize < 1) return 0;
@@ -1426,6 +1481,7 @@ template <class W, int V> LZ_HD int decode_unit(const u8* src, u32 csize_u, u8* 
             else lanes_copy<W>(dst + op, src + ip, len);
             W::sync();
             op += len; ip += len;
+            if (kPartial && op >= (long)target) break;
             continue;
         }
         if (hdr & kFlagLen) return -1;
@@ -1448,10 +1504,12 @@ template <class W, int V> LZ_HD int decode_unit(const u8* src, u32 csize_u, u8* 
         if (!read_stream<W>(hdr & kFlagLiterals, src, csize, ip, scratch, &s.lits, &s.nlits, sh, pre_lits)) return -1;
         if (ip > csize) return -1;
         int res;
-        if (us != nullptr && ip0 == 1 && us->state == kPreDone) res = decode_block_from_records<W>(s, dst, (u32)op, us, recs, sh);
-        else res = lizv1 ? decode_tokens_lizv1<W, V>(s, dst, (u32)op, cap, sh) : decode_tokens_lz4<W, V>(s, dst, (u32)op, cap, sh);
+        if (!kPartial && us != nullptr && ip0 == 1 && us->state == kPreDone) res = decode_block_from_records<W>(s, dst, (u32)op, us, recs, sh);
+        else res = lizv1 ? decode_tokens_lizv1<W, V, kPartial>(s, dst, (u32)op, cap, sh, op + target)
+                         : decode_tokens_lz4<W, V, kPartial>(s, dst, (u32)op, cap, sh, op + target);
         if (res <= 0) return res;
         op += res;
+        if (kPartial && op >= (long)target) break;
     }
     return (int)op;
 }

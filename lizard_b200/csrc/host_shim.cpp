@@ -79,6 +79,21 @@ extern "C" int lzb_host_decompress(const unsigned char* src, int csize, unsigned
     return r;
 }
 
+// Lizard_decompress_safe_partial through the one-lane instantiation of the partial decoder (the schedule the device's
+// partial kernel runs, without pre-passes)
+extern "C" int lzb_host_decompress_partial(const unsigned char* src, int csize, unsigned char* dst, int target, int cap)
+{
+    if (csize < 1) return 0;
+    if (cap < 0) return -1;
+    unsigned char* scratch = (unsigned char*)malloc(lzb::kDecScratchPerWarp);
+    lzb::DecWarpShared* sh = (lzb::DecWarpShared*)malloc(sizeof(lzb::DecWarpShared));
+    sh->big_table = (lzb::u16*)(scratch + 4 * lzb::kDecStreamScratch);
+    const int r = lzb::decode_unit<lzb::HostLanes, 3, true>(src, (lzb::u32)csize, dst, (lzb::u32)cap, scratch, sh,
+                                                            nullptr, nullptr, nullptr, nullptr, target);
+    free(scratch); free(sh);
+    return r;
+}
+
 // The Huffman pre-pass (huf_expand.cuh) as the device runs it, serially: plan the unit's first inner block, expand the
 // planned streams into an arena with the same per-segment function, hand the result to the token decoder.
 struct HostPre { lzb::UnitPre up; unsigned char* arena; int jobs; };
@@ -325,6 +340,31 @@ extern "C" int lzb_emu_decompress(const unsigned char* src, int csize, unsigned 
     a.sh = (lzb::DecWarpShared*)malloc(sizeof(lzb::DecWarpShared));
     a.sh->big_table = (lzb::u16*)(a.scratch + 4 * lzb::kDecStreamScratch);
     emu::run(emu_decompress_body, &a);
+    free(a.scratch); free(a.sh);
+    return a.result;
+}
+
+struct EmuPartialArgs { const unsigned char* src; int csize; unsigned char* dst; int target; int cap; unsigned char* scratch;
+                        lzb::DecWarpShared* sh; int result; };
+static void emu_partial_body(void* p)
+{
+    EmuPartialArgs* a = (EmuPartialArgs*)p;
+    const int r = lzb::decode_unit<EmuLanes, 3, true>(a->src, (lzb::u32)a->csize, a->dst, (lzb::u32)a->cap, a->scratch, a->sh,
+                                                      nullptr, nullptr, nullptr, nullptr, a->target);
+    if (EmuLanes::lane() == 0) a->result = r;
+}
+
+// Lizard_decompress_safe_partial through the 32-lane emulation of the device's partial kernel
+extern "C" int lzb_emu_decompress_partial(const unsigned char* src, int csize, unsigned char* dst, int target, int cap)
+{
+    if (csize < 1) return 0;
+    if (cap < 0) return -1;
+    EmuPartialArgs a;
+    a.src = src; a.csize = csize; a.dst = dst; a.target = target; a.cap = cap; a.result = -1;
+    a.scratch = (unsigned char*)malloc(lzb::kDecScratchPerWarp);
+    a.sh = (lzb::DecWarpShared*)malloc(sizeof(lzb::DecWarpShared));
+    a.sh->big_table = (lzb::u16*)(a.scratch + 4 * lzb::kDecStreamScratch);
+    emu::run(emu_partial_body, &a);
     free(a.scratch); free(a.sh);
     return a.result;
 }
