@@ -44,9 +44,17 @@ def lib():
         L.LizardB200_decompress_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int]
         L.Lizard_decompress_safe_partial.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.LizardB200_decompress_partial_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, c_int_p, ctypes.c_int]
+        L.Lizard_decompress_safe_usingDict.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                       ctypes.c_void_p, ctypes.c_int]
+        L.Lizard_createStreamDecode.restype = ctypes.c_void_p
+        L.Lizard_freeStreamDecode.argtypes = [ctypes.c_void_p]
+        L.Lizard_setStreamDecode.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
+        L.Lizard_decompress_safe_continue.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
+        L.LizardB200_decompress_dict_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int]
         dev_args = [ctypes.c_void_p] * 7 + [ctypes.c_uint]
         L.LizardB200_decompress_device.argtypes = dev_args + [ctypes.c_void_p]
         L.LizardB200_decompress_partial_device.argtypes = [ctypes.c_void_p] * 8 + [ctypes.c_uint, ctypes.c_void_p]
+        L.LizardB200_decompress_dict_device.argtypes = [ctypes.c_void_p] * 10 + [ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_compress_device.argtypes = dev_args + [ctypes.c_int, ctypes.c_void_p]
         L.LizardB200_gather_device.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_compress_blocks.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p,
@@ -92,7 +100,23 @@ def decompress_partial(src: bytes, target: int, max_size: int):
     return r, (dst.raw[:r] if r > 0 else b"")
 
 
-def _batch(fn, units, caps, extra, targets=None):
+def decompress_using_dict(src: bytes, dict: bytes, max_size: int, prefix: bool = False):
+    """Lizard_decompress_safe_usingDict on host bytes -> (return code, bytes).  prefix=True lays the dictionary directly in
+    front of the output buffer (the reference's in-place mode); otherwise it is an external dictionary."""
+    L = lib()
+    if prefix:
+        buf = ctypes.create_string_buffer(bytes(dict), len(dict) + max(max_size, 1))
+        dict_p, dst_p = ctypes.addressof(buf), ctypes.addressof(buf) + len(dict)
+    else:
+        d = ctypes.create_string_buffer(bytes(dict), max(len(dict), 1))
+        buf = ctypes.create_string_buffer(max(max_size, 1))
+        dict_p, dst_p = ctypes.addressof(d), ctypes.addressof(buf)
+    r = L.Lizard_decompress_safe_usingDict(src, dst_p, len(src), max_size, dict_p, len(dict))
+    out = ctypes.string_at(dst_p, r) if r > 0 else b""
+    return r, out
+
+
+def _batch(fn, units, caps, extra, targets=None, dicts=None):
     n = len(units)
     srcs = (ctypes.c_void_p * n)()
     sizes = (ctypes.c_int * n)()
@@ -109,10 +133,12 @@ def _batch(fn, units, caps, extra, targets=None):
         outs.append(o)
         dsts[i] = ctypes.cast(o, ctypes.c_void_p)
         dcaps[i] = caps[i]
-    if targets is None:
-        st = fn(srcs, sizes, dsts, dcaps, res, n, *extra)
-    else:
+    if targets is not None:
         st = fn(srcs, sizes, dsts, dcaps, (ctypes.c_int * n)(*targets), res, n, *extra)
+    elif dicts is not None:
+        st = fn(srcs, sizes, dsts, dcaps, dicts[0], dicts[1], res, n, *extra)
+    else:
+        st = fn(srcs, sizes, dsts, dcaps, res, n, *extra)
     _check(st, "batch call")
     return [(res[i], outs[i].raw[:res[i]] if res[i] > 0 else b"") for i in range(n)]
 
@@ -135,6 +161,23 @@ def decompress_partial_batch(units, targets, caps):
     if len(targets) != len(units):
         raise ValueError("one target per unit")
     return _batch(lib().LizardB200_decompress_partial_batch, units, caps, (), targets)
+
+
+def decompress_dict_batch(units, dicts, caps):
+    """LizardB200_decompress_dict_batch: list of compressed bytes, per-unit dictionary (bytes; b"" or None for none) and
+    capacity -> list of (result, bytes), each as decompress_using_dict with an external dictionary.  Units given the same
+    bytes object share one dictionary buffer."""
+    if len(dicts) != len(units):
+        raise ValueError("one dictionary per unit")
+    n = len(units)
+    ptrs, sizes, held = (ctypes.c_void_p * n)(), (ctypes.c_int * n)(), {}
+    for i, d in enumerate(dicts):
+        if d:
+            if id(d) not in held:
+                held[id(d)] = ctypes.create_string_buffer(bytes(d), len(d))
+            ptrs[i] = ctypes.addressof(held[id(d)])
+            sizes[i] = len(d)
+    return _batch(lib().LizardB200_decompress_dict_batch, units, caps, (), dicts=(ptrs, sizes))
 
 
 def _load_dg():

@@ -11,6 +11,8 @@
 #include <thread>
 #include <functional>
 #include <vector>
+#include <unordered_map>
+#include <utility>
 #include <string>
 #include <atomic>
 #include <cstring>
@@ -34,7 +36,8 @@ constexpr int kMaxDevices = 16;
 
 // Body of the first-generation decode kernels: a persistent set of warps, one unit per warp at a time.
 // kPartial: Lizard_decompress_safe_partial with the unit's b.target instead of Lizard_decompress_safe.
-template <int V, bool kPartial> __device__ __forceinline__ void decode_units(const DecodeBatch& b)
+// kDict: Lizard_decompress_safe_usingDict with the unit's dictionary (b.dict_*).
+template <int V, bool kPartial, bool kDict = false> __device__ __forceinline__ void decode_units(const DecodeBatch& b)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const u32 warp = threadIdx.x >> 5, lane = WarpLanes::lane();
@@ -58,6 +61,16 @@ template <int V, bool kPartial> __device__ __forceinline__ void decode_units(con
         if constexpr (kPartial) r = decode_unit<WarpLanes, V, true>(b.src_base + b.src_off[unit], b.src_len[unit],
                                                           b.dst_base + b.dst_off[unit], b.dst_cap[unit], scratch, sh,
                                                           nullptr, nullptr, nullptr, nullptr, b.target[unit]);
+        else if constexpr (kDict) {
+            u8* const dst = b.dst_base + b.dst_off[unit];
+            const u32 dl = b.dict_len[unit];
+            DictWin dw;
+            dw.end = b.dict_base + b.dict_off[unit] + dl;
+            dw.avail = dl;
+            dw.reach = b.dict_reach ? b.dict_reach[unit] : dict_reach(dl, dw.end == dst);
+            r = decode_unit<WarpLanes, V, false, true>(b.src_base + b.src_off[unit], b.src_len[unit], dst, b.dst_cap[unit], scratch, sh,
+                                                       b.pre ? b.pre + unit : nullptr, b.arena, nullptr, nullptr, 0, dw);
+        }
         else r = decode_unit<WarpLanes, V>(b.src_base + b.src_off[unit], b.src_len[unit],
                                            b.dst_base + b.dst_off[unit], b.dst_cap[unit], scratch, sh,
                                            b.pre ? b.pre + unit : nullptr, b.arena,
@@ -78,10 +91,18 @@ lizard_decode_units_kernel(DecodeBatch b)
 
 // Partial decode (LizardB200_decompress_partial_*): a kernel of its own, so that the full decode above keeps its code.  It runs
 // the default schedule and never the pre-passes, which expand or parse whole streams that a partial unit may never reach.
-constexpr int kDecPartialSchedule = 3;
+constexpr int kDecDefaultSchedule = 3;
 __global__ void __launch_bounds__(kDecWarps * 32, 4) lizard_decode_partial_units_kernel(DecodeBatch b)
 {
-    decode_units<kDecPartialSchedule, true>(b);
+    decode_units<kDecDefaultSchedule, true>(b);
+}
+
+// Decoding against dictionaries (LizardB200_decompress_dict_*, Lizard_decompress_safe_usingDict / _continue): a kernel of its
+// own as well, on the default schedule.  The Huffman pre-pass may run ahead of it (it reads only the compressed streams); the
+// token pre-pass and the second generation never do, whatever the decode variant: both check offsets against the unit start.
+__global__ void __launch_bounds__(kDecWarps * 32, 4) lizard_decode_dict_units_kernel(DecodeBatch b)
+{
+    decode_units<kDecDefaultSchedule, false, true>(b);
 }
 
 // Variable-length segments to their places in another arena (segment i: src_off[i], len[i] -> dst_off[i]): what the frame
@@ -189,7 +210,7 @@ struct Context {
     bool ready = false, failed = false;
     int device = 0, sm_count = 0;
     cudaStream_t stream = nullptr, s_in = nullptr, s_out = nullptr;   // compute / H2D / D2H
-    int decp_grid = 0;                        // grid of the partial-decode kernel
+    int decp_grid = 0, decd_grid = 0;         // grids of the partial-decode and dictionary-decode kernels
     int dec_grid = 0, dec_variant = 7;        // bits 0-1: schedule of the token loops, bit 2: Huffman pre-pass, bit 3: token pre-pass,
                                               // bit 4: second-generation kernel (parser + copier warp per unit)
     int dec2_grid = 0, dec2_stages = 4;
@@ -291,16 +312,20 @@ int ensure_context(Context& c, int device)
     for (int v = 0; v < 4; ++v)
         cudaFuncSetAttribute(decode_kernel(v), cudaFuncAttributePreferredSharedMemoryCarveout,
                              carveout((size_t)per_sm * (dec_smem + 1024), "LIZARDB200_DEC_CARVEOUT"));
-    {   // partial decode: same launch shape and scratch as the full decode, its own kernel
-        int pp = 0;
-        e = cudaFuncSetAttribute(lizard_decode_partial_units_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec_smem);
-        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pp, lizard_decode_partial_units_kernel, kDecWarps * 32, dec_smem);
-        if (e != cudaSuccess) { c.failed = true; fail("cudaFuncSetAttribute(partial decode)", e); return LIZARDB200_ERR_CUDA; }
-        if (pp < 1) pp = 1;
-        if (pp > per_sm) pp = per_sm;                 // the scratch below is sized for dec_grid
-        c.decp_grid = c.sm_count * pp;
-        cudaFuncSetAttribute(lizard_decode_partial_units_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                             carveout((size_t)pp * (dec_smem + 1024), "LIZARDB200_DEC_CARVEOUT"));
+    {   // partial and dictionary decode: same launch shape and scratch as the full decode, kernels of their own
+        const DecodeKernel own[2] = { lizard_decode_partial_units_kernel, lizard_decode_dict_units_kernel };
+        int* const grid[2] = { &c.decp_grid, &c.decd_grid };
+        for (int k = 0; k < 2; ++k) {
+            int pp = 0;
+            e = cudaFuncSetAttribute(own[k], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec_smem);
+            if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pp, own[k], kDecWarps * 32, dec_smem);
+            if (e != cudaSuccess) { c.failed = true; fail("cudaFuncSetAttribute(partial / dictionary decode)", e); return LIZARDB200_ERR_CUDA; }
+            if (pp < 1) pp = 1;
+            if (pp > per_sm) pp = per_sm;             // the scratch below is sized for dec_grid
+            *grid[k] = c.sm_count * pp;
+            cudaFuncSetAttribute(own[k], cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 carveout((size_t)pp * (dec_smem + 1024), "LIZARDB200_DEC_CARVEOUT"));
+        }
     }
     {   // second generation: CTAs of two warps, static shared memory; as many per SM as fit (LIZARDB200_DEC2_CTAS_PER_SM caps it)
         if (const char* v = getenv("LIZARDB200_DEC2_STAGES")) c.dec2_stages = atoi(v) >= 8 ? 8 : 4;
@@ -490,6 +515,35 @@ int launch_decode_partial(Context& c, const void* dSrc, const u64* dSrcOff, cons
     return LIZARDB200_OK;
 }
 
+// Lizard_decompress_safe_usingDict for every unit against the dictionary dDictLen[i] bytes at dDict + dDictOff[i]: one launch
+// of the dictionary kernel, behind the Huffman pre-pass under the rule of launch_decode.  dDictReach: see DecodeBatch.
+int launch_decode_dict(Context& c, const void* dSrc, const u64* dSrcOff, const u32* dSrcLen,
+                       void* dDst, const u64* dDstOff, const u32* dDstCap, const void* dDict, const u64* dDictOff,
+                       const u32* dDictLen, const u32* dDictReach, int* dResult, u32 n, cudaStream_t s)
+{
+    if (n == 0) return LIZARDB200_OK;
+    workspace_acquire(c, s);
+    struct Release { Context& c; cudaStream_t s; ~Release() { workspace_release(c, s); } } release_on_exit{c, s};
+    DecodeBatch b;
+    memset(&b, 0, sizeof b);
+    b.src_base = (const u8*)dSrc; b.src_off = dSrcOff; b.src_len = dSrcLen;
+    b.dst_base = (u8*)dDst; b.dst_off = dDstOff; b.dst_cap = dDstCap;
+    b.result = dResult; b.n_units = n;
+    b.dict_base = (const u8*)dDict; b.dict_off = dDictOff; b.dict_len = dDictLen; b.dict_reach = dDictReach;
+    b.scratch = (u8*)c.dec_scratch.p;
+    b.counter = next_counter(c, s);
+    if ((c.dec_variant & 4) && n >= kPrepassMinUnits) {
+        int st = launch_prepass(c, b, s);
+        if (st != LIZARDB200_OK) return st;
+    }
+    int grid = (int)((n + kDecWarps - 1) / kDecWarps);
+    if (grid > c.decd_grid) grid = c.decd_grid;
+    lizard_decode_dict_units_kernel<<<grid, kDecWarps * 32, sizeof(DecWarpShared) * kDecWarps, s>>>(b);
+    g_launches++;
+    CU_OK(cudaGetLastError());
+    return LIZARDB200_OK;
+}
+
 int launch_encode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* dSrcLen,
                   void* dDst, const u64* dDstOff, const u32* dDstCap, int* dResult, u32 n, int level, cudaStream_t s,
                   const Progress* pg = nullptr, const FramePack* fp = nullptr)
@@ -518,9 +572,13 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // Shared body of the host-pointer batch calls: stage inputs + tables, run, fetch results + outputs.
 // `target` (decode only): per-unit targetOutputSize of a partial decode, null for a full one.
+// `dict` / `dictSize` (decode only): per-unit dictionary of Lizard_decompress_safe_usingDict, null for none.  Only the bytes
+// a unit's matches can reach are staged (dict_window of its level), once per dictionary end address; a negative size gives
+// the unit -1 without decoding it.  `dictReach`: the units' reaches, if not the ones their dictionaries imply (_continue).
 template <bool kCompress>
 int run_host_batch(const void* const* src, const int* srcSize, void* const* dst, const int* dstCap,
-                   int* result, int n, int level, const int* target = nullptr)
+                   int* result, int n, int level, const int* target = nullptr,
+                   const void* const* dict = nullptr, const int* dictSize = nullptr, const u32* dictReach = nullptr)
 {
     if (n < 0 || (n > 0 && (!src || !srcSize || !dst || !dstCap || !result))) return LIZARDB200_ERR_ARGUMENT;
     if (n == 0) return LIZARDB200_OK;
@@ -541,7 +599,35 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
         in_off[i] = in_total;   in_total += align_up((size_t)srcSize[i] + 16, 16);
         out_off[i] = out_total; out_total += align_up((size_t)dstCap[i] + 32, 16);
     }
-    const size_t tab_bytes = (size_t)n * (8 + 4 + 8 + 4 + (target ? 4 : 0) + 4);
+    // dictionaries go behind the inputs, one staged copy per dictionary end address, as long as the longest reach of a unit
+    // that uses it
+    const int nd = dict ? n : 0;
+    std::vector<u32> dict_avail(nd), dict_rch(nd);
+    std::vector<u64> dict_at(nd);                                 // arena offset of unit i's first readable dictionary byte
+    struct Staged { const u8* end; u32 bytes; u64 at; };
+    std::vector<Staged> staged;
+    if (dict) {
+        std::unordered_map<const u8*, size_t> slot;
+        std::vector<size_t> unit_slot(n);
+        for (int i = 0; i < n; ++i) {
+            dict_avail[i] = dict_rch[i] = 0; dict_at[i] = 0;
+            if (dictSize[i] <= 0 || srcSize[i] < 1) continue;
+            if (!dict[i]) return LIZARDB200_ERR_ARGUMENT;
+            const u8* end = (const u8*)dict[i] + dictSize[i];
+            const int lv = ((const u8*)src[i])[0];
+            const u32 win = (lv >= (int)kMinLevel && lv <= (int)kMaxLevel) ? dict_window(lv) : 0u;
+            dict_avail[i] = (u32)dictSize[i] < win ? (u32)dictSize[i] : win;
+            dict_rch[i] = dictReach ? dictReach[i] : dict_reach((u32)dictSize[i], end == (const u8*)dst[i]);
+            auto it = slot.find(end);
+            if (it == slot.end()) { it = slot.emplace(end, staged.size()).first; staged.push_back(Staged{end, 0, 0}); }
+            unit_slot[i] = it->second;
+            if (staged[it->second].bytes < dict_avail[i]) staged[it->second].bytes = dict_avail[i];
+        }
+        for (Staged& d : staged) { d.at = in_total; in_total = align_up(in_total + d.bytes + 16, 16); }
+        for (int i = 0; i < n; ++i)
+            if (dict_avail[i]) { const Staged& d = staged[unit_slot[i]]; dict_at[i] = d.at + d.bytes - dict_avail[i]; }
+    }
+    const size_t tab_bytes = (size_t)n * (8 + 4 + 8 + 4 + (target ? 4 : 0) + (dict ? 8 + 4 + 4 : 0) + 4);
     CU_OK(c.pin_in.reserve(in_total));
     CU_OK(c.pin_tab.reserve(tab_bytes));
     CU_OK(c.d_in.reserve(in_total));
@@ -554,14 +640,19 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
     u64* t_out_off = t_in_off + n;
     u32* t_in_len = (u32*)(t_out_off + n);
     u32* t_out_cap = t_in_len + n;
-    int* t_target = (int*)(t_out_cap + n);
+    u64* t_dict_off = (u64*)(t_out_cap + n);                      // 8-byte aligned: 24 bytes per unit in front of it
+    u32* t_dict_len = (u32*)(t_dict_off + nd);
+    u32* t_dict_reach = t_dict_len + nd;
+    int* t_target = (int*)(t_dict_reach + nd);
     int* t_res = t_target + (target ? n : 0);
     for (int i = 0; i < n; ++i) {
         memcpy((u8*)c.pin_in.p + in_off[i], src[i], (size_t)srcSize[i]);
         t_in_off[i] = in_off[i]; t_out_off[i] = out_off[i];
         t_in_len[i] = (u32)srcSize[i]; t_out_cap[i] = (u32)dstCap[i];
         if (target) t_target[i] = target[i];
+        if (dict) { t_dict_off[i] = dict_at[i]; t_dict_len[i] = dict_avail[i]; t_dict_reach[i] = dict_rch[i]; }
     }
+    for (const Staged& d : staged) memcpy((u8*)c.pin_in.p + d.at, d.end - d.bytes, d.bytes);
     u8* dtab = (u8*)c.d_tab.p;
     cudaStream_t s = c.stream;
     CU_OK(cudaMemcpyAsync(c.d_in.p, c.pin_in.p, in_total, cudaMemcpyHostToDevice, s));
@@ -570,18 +661,23 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
     const u64* d_out_off = d_in_off + n;
     const u32* d_in_len = (const u32*)(d_out_off + n);
     const u32* d_out_cap = d_in_len + n;
-    const int* d_target = (const int*)(d_out_cap + n);
+    const u64* d_dict_off = (const u64*)(d_out_cap + n);
+    const u32* d_dict_len = (const u32*)(d_dict_off + nd);
+    const u32* d_dict_reach = d_dict_len + nd;
+    const int* d_target = (const int*)(d_dict_reach + nd);
     int* d_res = (int*)d_target + (target ? n : 0);
     if (kCompress) st = launch_encode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, level, s);
     else if (target) st = launch_decode_partial(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_target, d_res, (u32)n, s);
+    else if (dict) st = launch_decode_dict(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, c.d_in.p, d_dict_off,
+                                           d_dict_len, d_dict_reach, d_res, (u32)n, s);
     else           st = launch_decode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, s);
     if (st != LIZARDB200_OK) return st;
     CU_OK(cudaMemcpyAsync(t_res, d_res, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
     CU_OK(cudaMemcpyAsync(c.pin_out.p, c.d_out.p, out_total, cudaMemcpyDeviceToHost, s));
     CU_OK(cudaStreamSynchronize(s));
     for (int i = 0; i < n; ++i) {
-        result[i] = t_res[i];
-        if (t_res[i] > 0) memcpy(dst[i], (u8*)c.pin_out.p + out_off[i], (size_t)t_res[i]);
+        result[i] = dict && dictSize[i] < 0 ? -1 : t_res[i];
+        if (result[i] > 0) memcpy(dst[i], (u8*)c.pin_out.p + out_off[i], (size_t)t_res[i]);
     }
     return LIZARDB200_OK;
 }
@@ -675,6 +771,19 @@ int LizardB200_decompress_partial_device(const void* dSrc, const uint64_t* dSrcO
     return launch_decode_partial(c, dSrc, (const u64*)dSrcOff, dSrcLen, dDst, (const u64*)dDstOff, dDstCap, dTarget, dResult, nUnits,
                                  (cudaStream_t)stream);
 }
+int LizardB200_decompress_dict_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
+                                      void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
+                                      const void* dDict, const uint64_t* dDictOff, const uint32_t* dDictLen,
+                                      int* dResult, unsigned nUnits, void* stream)
+{
+    if (nUnits > 0 && (!dDictOff || !dDictLen)) return LIZARDB200_ERR_ARGUMENT;
+    Context& c = g_ctx[g_device];
+    std::lock_guard<std::mutex> lock(c.mu);
+    int st = ensure_context(c, g_device);
+    if (st != LIZARDB200_OK) return st;
+    return launch_decode_dict(c, dSrc, (const u64*)dSrcOff, dSrcLen, dDst, (const u64*)dDstOff, dDstCap, dDict, (const u64*)dDictOff,
+                              dDictLen, nullptr, dResult, nUnits, (cudaStream_t)stream);
+}
 int LizardB200_compress_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
                                void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
                                int* dResult, unsigned nUnits, int level, void* stream)
@@ -713,6 +822,12 @@ int LizardB200_decompress_partial_batch(const void* const* src, const int* cSize
 {
     if (n > 0 && !targetOutputSize) return LIZARDB200_ERR_ARGUMENT;
     return run_host_batch<false>(src, cSize, dst, dstCap, result, n, 0, targetOutputSize);
+}
+int LizardB200_decompress_dict_batch(const void* const* src, const int* cSize, void* const* dst, const int* dstCap,
+                                     const void* const* dict, const int* dictSize, int* result, int n)
+{
+    if (n > 0 && (!dict || !dictSize)) return LIZARDB200_ERR_ARGUMENT;
+    return run_host_batch<false>(src, cSize, dst, dstCap, result, n, 0, nullptr, dict, dictSize);
 }
 int LizardB200_compress_batch(const void* const* src, const int* srcSize, void* const* dst, const int* dstCap,
                               int* result, int n, int level)
@@ -833,12 +948,16 @@ int Lizard_compress_extState(void* state, const char* src, char* dst, int srcSiz
 // ---- the rest of lib/dll/liblizard.def: what callers of the block API link against -------------------------------------
 // Stream OBJECTS are functional (the reference's frame layer creates one per context and hands it to
 // Lizard_compress_extState, lib/lizard_frame.c:379-401, 436-451); the device keeps the real state, so the object only
-// records its level.  The streaming / dictionary FAMILY (linked blocks, cross-call windows) is out of scope (SURVEY.md
-// section 2): those entry points exist so that the reference's own callers link, and they fail with the reference's
-// failure values -- 0 from the compress side, a negative value from the decode side -- never with a CPU code path.
+// records its level.  Dictionary and streamed DECODING run on the GPU (Lizard_decompress_safe_usingDict, _continue); the
+// compress side of the family (Lizard_loadDict, Lizard_saveDict, Lizard_compress_continue) is out of scope (SURVEY.md
+// section 2): those entry points exist so that the reference's own callers link, and they fail with the reference's failure
+// value 0, never with a CPU code path.
 struct Lizard_stream_s { size_t allocatedMemory; int compressionLevel; };
-struct Lizard_streamDecode_s { const char* dict; int dictSize; };
-static const char* const kNoStreaming = "streaming / dictionary API (linked blocks) is not implemented on the GPU path";
+struct Lizard_streamDecode_s {                                   // lib/lizard_common.h:195-200
+    const u8* externalDict; size_t extDictSize;
+    const u8* prefixEnd; size_t prefixSize;
+};
+static const char* const kNoStreaming = "streaming compression with a dictionary (linked blocks) is not implemented on the GPU path";
 
 Lizard_stream_t* Lizard_createStream(int level)            // lib/lizard_compress.c:392-397
 {
@@ -863,12 +982,60 @@ int Lizard_compress_continue(Lizard_stream_t*, const char*, char*, int, int) { g
 
 Lizard_streamDecode_t* Lizard_createStreamDecode(void) { return (Lizard_streamDecode_t*)calloc(1, sizeof(Lizard_streamDecode_t)); }
 int Lizard_freeStreamDecode(Lizard_streamDecode_t* p) { free(p); return 0; }
-int Lizard_setStreamDecode(Lizard_streamDecode_t* p, const char* dict, int dictSize)   // lib/lizard_decompress.c:303-319
+int Lizard_setStreamDecode(Lizard_streamDecode_t* p, const char* dict, int dictSize)   // lib/lizard_decompress.c:303-310
 {
-    if (p) { p->dict = dict; p->dictSize = dictSize; }
+    p->prefixSize = (size_t)dictSize;
+    p->prefixEnd = (const u8*)dict + dictSize;
+    p->externalDict = nullptr;
+    p->extDictSize = 0;
     return 1;
 }
-int Lizard_decompress_safe_continue(Lizard_streamDecode_t*, const char*, char*, int, int) { g_last_error = kNoStreaming; return -1; }
+
+namespace {
+// One unit against the window [ext, ext + extSize) followed by [pre, pre + preSize) in front of dst (the window of
+// Lizard_decompress_safe_continue, lib/lizard_decompress.c:322-344): the bytes its matches can reach are gathered into one
+// buffer and decoded as an external dictionary whose reach is the whole window.
+int decompress_window(const char* src, char* dst, int compressedSize, int maxOut, const u8* ext, size_t extSize,
+                      const u8* pre, size_t preSize)
+{
+    if (compressedSize < 1) return 0;
+    if (maxOut < 0) return -1;
+    const int lv = (u8)src[0];
+    const size_t total = extSize + preSize;
+    const size_t win = (lv >= (int)kMinLevel && lv <= (int)kMaxLevel) ? dict_window(lv) : 0;
+    const size_t keep = total < win ? total : win;
+    std::vector<u8> buf(keep + 1);
+    const size_t from_pre = keep < preSize ? keep : preSize, from_ext = keep - from_pre;
+    if (from_ext) memcpy(buf.data(), ext + extSize - from_ext, from_ext);
+    if (from_pre) memcpy(buf.data() + from_ext, pre + preSize - from_pre, from_pre);
+    // the reference checks offsets against the whole window unless the external part alone is 2^24 bytes or more; from a
+    // window of 2^24 bytes on no offset can fail the check either
+    const u32 reach = total >= ((size_t)1 << 24) ? kDictUnchecked : (u32)total;
+    const void* s = src; void* d = dst; const void* dict = buf.data(); const int dsize = (int)keep; int r = -1;
+    int st = run_host_batch<false>(&s, &compressedSize, &d, &maxOut, &r, 1, 0, nullptr, &dict, &dsize, &reach);
+    return st == LIZARDB200_OK ? r : st;
+}
+}  // namespace
+
+int Lizard_decompress_safe_continue(Lizard_streamDecode_t* p, const char* src, char* dst, int compressedSize, int maxOutputSize)
+{
+    int r;
+    if (p->prefixEnd == (const u8*)dst) {
+        r = decompress_window(src, dst, compressedSize, maxOutputSize, p->externalDict, p->extDictSize,
+                              p->prefixEnd - p->prefixSize, p->prefixSize);
+        if (r <= 0) return r;
+        p->prefixSize += (size_t)r;
+        p->prefixEnd += r;
+    } else {
+        p->extDictSize = p->prefixSize;
+        p->externalDict = p->prefixEnd - p->extDictSize;
+        r = decompress_window(src, dst, compressedSize, maxOutputSize, p->externalDict, p->extDictSize, nullptr, 0);
+        if (r <= 0) return r;
+        p->prefixSize = (size_t)r;
+        p->prefixEnd = (const u8*)dst + r;
+    }
+    return r;
+}
 int Lizard_decompress_safe_partial(const char* src, char* dst, int compressedSize, int targetOutputSize, int maxDecompressedSize)
 {
     // same argument handling as Lizard_decompress_safe (lib/lizard_decompress.c:139, 272-275)
@@ -881,11 +1048,14 @@ int Lizard_decompress_safe_partial(const char* src, char* dst, int compressedSiz
 int Lizard_decompress_safe_usingDict(const char* src, char* dst, int compressedSize, int maxDecompressedSize,
                                      const char* dictStart, int dictSize)
 {
-    // lib/lizard_decompress.c:353-355: without a dictionary this is Lizard_decompress_safe
+    // lib/lizard_decompress.c:351-360: without a dictionary this is Lizard_decompress_safe
     if (dictSize == 0) return Lizard_decompress_safe(src, dst, compressedSize, maxDecompressedSize);
-    (void)dictStart;
-    g_last_error = kNoStreaming;
-    return -1;
+    if (dictSize < 0) return -1;
+    if (compressedSize < 1) return 0;
+    if (maxDecompressedSize < 0) return -1;
+    const void* s = src; void* d = dst; const void* dict = dictStart; int r = -1;
+    int st = LizardB200_decompress_dict_batch(&s, &compressedSize, &d, &maxDecompressedSize, &dict, &dictSize, &r, 1);
+    return st == LIZARDB200_OK ? r : st;
 }
 
 }  // extern "C"

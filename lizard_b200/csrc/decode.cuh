@@ -95,7 +95,41 @@ struct DecodeBatch {
     const UnitSeq* seq;     // [n] blocks parsed by the token pre-pass, or null
     const PoolRun* recs;    // its sequence records
     const int* target;      // [n] targetOutputSize of a partial decode (lizard_decode_partial_units_kernel), null for a full one
+    // decoding against dictionaries (lizard_decode_dict_units_kernel): unit i's dictionary is the dict_len[i] bytes at
+    // dict_base + dict_off[i] (dict_len[i] == 0: none).  dict_reach null: the reach follows from dict_len and the prefix test
+    // (dictionary end == the unit's output), as in Lizard_decompress_safe_usingDict; otherwise dict_reach[i] is the reach of
+    // a dictionary that was staged shorter than the caller's (see DictWin)
+    const u8*  dict_base;
+    const u64* dict_off;
+    const u32* dict_len;
+    const u32* dict_reach;
 };
+
+// ---- decoding against a dictionary (Lizard_decompress_safe_usingDict / _continue, lib/lizard_decompress.c:322-360) ----
+// A unit sees the `avail` bytes in front of `end` as the bytes in front of its own start: `end` is the dictionary's end
+// (the unit's own output in the reference's prefix mode, where the dictionary lies in place in front of it).  A match may
+// start up to `reach` bytes below the unit start before the reference's offset check (lowLimit = lowPrefix - dictSize)
+// rejects it; kDictUnchecked = the reference's checkOffset is off.  No match starts more than 65535 (fastLZ4 codewords) or
+// 2^24 - 1 (LIZv1) bytes below the unit start, so `avail` may be shorter than the caller's dictionary; `reach` may not.
+struct DictWin { const u8* end; u32 avail; u32 reach; };
+enum : u32 { kDictUnchecked = 0xffffffffu, kDictPrefixMax = (1u << 24) - 1 };
+// the reach of a dictionary of `size` bytes, `prefix` = it ends where the output starts (lib/lizard_decompress.c:349-360 picks
+// noDict with lowPrefix = dest - size, or withPrefix64k with lowPrefix = dest - 2^24 from size 2^24 - 1 on; usingExtDict
+// checks offsets only below size 2^24)
+LZ_HD u32 dict_reach(u32 size, bool prefix)
+{
+    if (prefix) return size >= kDictPrefixMax ? (1u << 24) : size;
+    return size >= (1u << 24) ? kDictUnchecked : size;
+}
+// farthest any match of a unit at this level starts below the unit start
+LZ_HD u32 dict_window(int level) { return level_is_lizv1(level) ? kDictPrefixMax : 65535u; }
+
+#if defined(LZB_DICT_STATS) && !defined(__CUDA_ARCH__)
+static unsigned long long g_dict_only = 0, g_dict_straddle = 0;      // matches read from the dictionary alone / across its end
+#define LZB_COUNT_DICT(only, straddle) (g_dict_only += (only), g_dict_straddle += (straddle))
+#else
+#define LZB_COUNT_DICT(only, straddle)
+#endif
 
 enum : u32 { kDecStreamScratch = kBlockSize + 64, kDecBigTableBytes = 2u << kHufTableLogMax,
              kDecScratchPerWarp = 4 * kDecStreamScratch + kDecBigTableBytes };
@@ -136,6 +170,18 @@ template <class W> LZ_HD void lanes_match(u8* dst, long op, u32 off, u32 len)
     else if (off != 0) { for (u32 i = W::lane(); i < len; i += W::lanes()) d[i] = s[i % off]; }
     else { for (u32 i = W::lane(); i < len; i += W::lanes()) d[i] = 0; }     // offset 0 (no encoder emits it; the reference copies
                                                                               // whatever dst held): defined output, nothing stale leaks
+}
+// The same match of a unit decoded against a dictionary: a source below the unit start reads the dictionary, and a match
+// that runs past the dictionary's end continues from the unit start with LZ77 overlap (lizard_decompress_lz4.h:99-121), the
+// bytes [dict][unit] read as one window.
+template <class W> LZ_HD void dict_match(u8* dst, long op, u32 off, u32 len, const DictWin& dw)
+{
+    if ((long)off <= op) { lanes_match<W>(dst, op, off, len); return; }
+    const u32 below = (u32)((long)off - op);
+    const u32 head = len < below ? len : below;
+    for (u32 i = W::lane(); i < head; i += W::lanes()) dst[op + i] = dw.end[(long)i - (long)below];
+    LZB_COUNT_DICT(W::lane() == 0 && len <= below ? 1 : 0, W::lane() == 0 && len > below ? 1 : 0);
+    if (len > below) { W::sync(); lanes_match<W>(dst, (long)off, off, len - below); }
 }
 
 // ---- Huffman stream expansion -----------------------------------------------------------------
@@ -524,9 +570,12 @@ struct TokCursor { u32 fp; long lp; long op; u32 p16, p24; u32 last_off; };
 // ---- serial path: the reference's loop, one token at a time (all lanes in lock step) ------------------
 // Returns 0 to continue, or the (negative) error code.  Runs at most `count` tokens.
 // kPartial (Lizard_decompress_safe_partial): returns 1 when the reference's loop stops at `oexit`, with c.op where it stopped.
-template <class W, bool kPartial = false> LZ_HD int lz4_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count, long oexit = 0)
+// kDict: matches may reach into the dictionary `dw` (c.op is the position in the unit, so offsets up to c.op + dw.reach pass).
+template <class W, bool kPartial = false, bool kDict = false>
+LZ_HD int lz4_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count, long oexit = 0, DictWin dw = DictWin())
 {
     const long nl = (long)s.nlits;
+    const long reach = kDict ? (long)dw.reach : 0;
     for (u32 t = 0; t < count && c.fp < s.nflags; ++t) {
         const u32 tok = s.flags[c.fp++];
         u32 len = tok & 15;
@@ -539,7 +588,7 @@ template <class W, bool kPartial = false> LZ_HD int lz4_serial(const Streams& s,
         c.op += len; c.lp += len;
         if (kPartial && c.op >= oexit) { W::sync(); return 1; }    // lizard_decompress_lz4.h:82, before the offset is read
         const u32 off = rd_le16(s.lits + c.lp); c.lp += 2;
-        if ((long)off > c.op) return -(int)c.fp - 1;               // match < lowLimit
+        if ((long)off > c.op + reach) return -(int)c.fp - 1;       // match < lowLimit
         u32 ml = tok >> 4;
         if (ml == 15) {
             if (c.lp > nl - 5) return -(int)c.fp - 1;
@@ -548,7 +597,8 @@ template <class W, bool kPartial = false> LZ_HD int lz4_serial(const Streams& s,
         ml += kMinMatch;
         if (c.op + ml > oend - 16) return -(int)c.fp - 1;
         W::sync();
-        lanes_match<W>(dst, c.op, off, ml);
+        if (kDict) dict_match<W>(dst, c.op, off, ml, dw);
+        else lanes_match<W>(dst, c.op, off, ml);
         W::sync();
         c.op += ml;
         if (kPartial && c.op >= oexit) return 1;                    // :144, the block's last literals are not copied
@@ -556,9 +606,11 @@ template <class W, bool kPartial = false> LZ_HD int lz4_serial(const Streams& s,
     return 0;
 }
 
-template <class W, bool kPartial = false> LZ_HD int lizv1_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count, long oexit = 0)
+template <class W, bool kPartial = false, bool kDict = false>
+LZ_HD int lizv1_serial(const Streams& s, u8* dst, long oend, TokCursor& c, u32 count, long oexit = 0, DictWin dw = DictWin())
 {
     const long nl = (long)s.nlits;
+    const long reach = kDict ? (long)dw.reach : 0;
     for (u32 t = 0; t < count && c.fp < s.nflags; ++t) {
         if (kPartial && c.op >= oexit) return 1;                    // lizard_decompress_liz.h:55, before the flags byte is read
         const u32 tok = s.flags[c.fp++];
@@ -596,10 +648,11 @@ template <class W, bool kPartial = false> LZ_HD int lizv1_serial(const Streams& 
             if ((long)c.p24 > (long)s.noff24 - 3) return -(int)c.fp - 1;
             c.last_off = rd_le24(s.off24 + c.p24); c.p24 += 3;
         }
-        if ((long)c.last_off > c.op) return -(int)c.fp - 1;         // match < lowLimit
+        if ((long)c.last_off > c.op + reach) return -(int)c.fp - 1; // match < lowLimit
         if (c.op + ml > oend - 16) return -(int)c.fp - 1;
         W::sync();
-        lanes_match<W>(dst, c.op, c.last_off, ml);
+        if (kDict) dict_match<W>(dst, c.op, c.last_off, ml, dw);
+        else lanes_match<W>(dst, c.op, c.last_off, ml);
         W::sync();
         c.op += ml;
     }
@@ -840,15 +893,22 @@ template <class W> LZ_HD void run_batch_copies(u8* dst, const u8* lits, u32 nb, 
 // into four pools -- short / long literal runs, short / long matches that read nothing a match of this batch writes --
 // and every pool is moved by one sweep that keeps all lanes busy (pool_copy_short / pool_copy_long, lanes.cuh).  Only
 // the matches that do read the output of an earlier match of the same batch (or themselves) follow one by one, in order.
-template <class W> LZ_HD void run_batch_copies_pool(u8* dst, const u8* lits, u32 nb, u32 lit_src, u32 lit_len,
-                                                    u32 opos, u32 off, u32 ml, PoolRun* pool)
+// kDict: a match may start below the unit start (off > its destination): one that lies wholly in the dictionary `dw` reads
+// nothing this batch writes and goes in a sweep of its own, one that runs past the dictionary's end goes in order.
+template <class W, bool kDict = false> LZ_HD void run_batch_copies_pool(u8* dst, const u8* lits, u32 nb, u32 lit_src, u32 lit_len,
+                                                                       u32 opos, u32 off, u32 ml, PoolRun* pool,
+                                                                       DictWin dw = DictWin())
 {
     typedef LaneGroups<W> LG;
     const u32 lane = W::lane(), L = W::lanes();
     const bool act = lane < nb;
     const u32 mdst = opos + lit_len;
     if (W::kLanes == 1) {                                   // one-lane host build: the reference's order
-        if (act) { for (u32 i = 0; i < lit_len; ++i) dst[opos + i] = lits[lit_src + i]; lanes_match<W>(dst, (long)mdst, off, ml); }
+        if (act) {
+            for (u32 i = 0; i < lit_len; ++i) dst[opos + i] = lits[lit_src + i];
+            if (kDict) dict_match<W>(dst, (long)mdst, off, ml, dw);
+            else lanes_match<W>(dst, (long)mdst, off, ml);
+        }
         return;
     }
     if (act && off != 0 && off <= mdst) W::prefetch(dst + (mdst - off));
@@ -866,8 +926,22 @@ template <class W> LZ_HD void run_batch_copies_pool(u8* dst, const u8* lits, u32
     W::sync();
     // A match is "free" when its source lies before the first match destination of this batch (older output, or the
     // first literal run), or inside ONE literal run of this batch: those bytes are final now.
-    const u32 msrc = mdst - off;                            // off <= mdst was checked by the caller
-    const bool real = act && ml != 0 && off != 0;
+    const u32 msrc = mdst - off;                            // off <= mdst was checked by the caller, unless kDict
+    const bool below = kDict && act && ml != 0 && off > mdst;
+    const bool dict_only = below && off - mdst >= ml;
+    const bool real = act && ml != 0 && off != 0 && !below;
+    if (kDict) {
+        const u32 sel_s = W::ballot(dict_only && ml <= LG::kMaxBytes), sel_l = W::ballot(dict_only && ml > LG::kMaxBytes);
+        if ((sel_s | sel_l) != 0) {
+            // positions relative to the lowest readable dictionary byte, so that they stay unsigned
+            const u8* const lo = dw.end - dw.avail;
+            const u32 from = dw.avail - (off - mdst);
+            pool_copy_short<W>(dst, lo, sel_s, mdst, from, ml, pool);
+            pool_copy_long<W>(dst, lo, sel_l, mdst, from, ml, pool + 32);
+            W::sync();                                      // the sweeps below reuse the pool
+        }
+        LZB_COUNT_DICT(lane == 0 ? popc32(sel_s | sel_l) : 0, 0);      // the others are counted by dict_match
+    }
     const u32 first = W::shfl(mdst, 0);
     bool free_m = real && msrc + ml <= first;
     {
@@ -878,14 +952,15 @@ template <class W> LZ_HD void run_batch_copies_pool(u8* dst, const u8* lits, u32
     }
     pool_copy_short<W>(dst, dst, W::ballot(free_m && ml <= LG::kMaxBytes), mdst, msrc, ml, pool);
     pool_copy_long<W>(dst, dst, W::ballot(free_m && ml > LG::kMaxBytes), mdst, msrc, ml, pool + 32);
-    u32 rest = W::ballot(act && ml != 0 && !free_m);
+    u32 rest = W::ballot(act && ml != 0 && !free_m && !dict_only);
     if (rest == 0) return;
     W::sync();
     for (; rest; rest &= rest - 1) {
         const u32 k = ctz32(rest);
         const u32 m = W::shfl(ml, k), o = W::shfl(off, k);
         u8* const to = dst + W::shfl(mdst, k);
-        if (m >= kWideMinBytes && o >= wide_min_offset<W>()) lanes_copy_wide<W>(to, to - o, m, true);
+        if (kDict && (long)o > (long)(to - dst)) dict_match<W>(dst, (long)(to - dst), o, m, dw);
+        else if (m >= kWideMinBytes && o >= wide_min_offset<W>()) lanes_copy_wide<W>(to, to - o, m, true);
         else if (o >= m || o >= 4 * L) {
             for (u32 base = 0; base < m; base += 4 * L) {
                 const u32 part = m - base < 4 * L ? m - base : 4 * L;
@@ -1081,10 +1156,13 @@ template <class W> LZ_HD bool ext_chain_win(const u8* lits, u32 nl, u32 lp, u32 
 // `oend` the unit's capacity; matches may reach back to offset 0 of the unit.
 // kPartial: the loop of Lizard_decompress_safe_partial, which returns as soon as the output reaches `oexit` (= op0 + the
 // target: the reference measures the target from the start of the inner block), after a token's literals or after its match.
-template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lz4(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh,
-                                                                   long oexit)
+// kDict: matches may reach into the dictionary `dw` (the default schedule only: the pooled sweeps read it).
+template <class W, int V, bool kPartial, bool kDict = false>
+LZ_HD int decode_tokens_lz4(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh, long oexit, DictWin dw = DictWin())
 {
+    static_assert(!kDict || (V & 1) != 0, "dictionary matches need the pooled copy sweeps");
     const long nl = (long)s.nlits, oend = (long)oend_u;
+    const long reach = kDict ? (long)dw.reach : 0;
     const u32 NL = W::lanes(), lane = W::lane();
     if (oend_u - op0 == 0) return (s.nflags == 1 && s.flags[0] == 0) ? 0 : -1;
     TokCursor c; c.fp = 0; c.lp = 0; c.op = op0; c.p16 = c.p24 = 0; c.last_off = 0;
@@ -1197,7 +1275,7 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lz4(const Strea
             if (act && !bad) {
                 if (opos + (long)lit_len > oend - 16) bad = true;
                 else if (kPartial && opos + (long)lit_len >= oexit) xl = true;
-                else if ((long)off > opos + (long)lit_len) bad = true;
+                else if ((long)off > opos + (long)lit_len + reach) bad = true;
                 else if (opos + (long)lit_len + (long)ml > oend - 16) bad = true;
                 else if (kPartial && opos + (long)lit_len + (long)ml >= oexit) xm = true;
             }
@@ -1212,7 +1290,7 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lz4(const Strea
                         if (xl) ml = 0;                                 // lane e: literals only; the lanes behind it do not run
                         const u32 end = W::shfl(O + lit_len + ml, e);
                         if ((V & 1) == 0) run_batch_copies<W>(dst, s.lits, e + 1, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
-                        else run_batch_copies_pool<W>(dst, s.lits, e + 1, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                        else run_batch_copies_pool<W, kDict>(dst, s.lits, e + 1, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc, dw);
                         W::sync();
                         return (int)(c.op + (long)end - (long)op0);
                     }
@@ -1225,13 +1303,13 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lz4(const Strea
                 asm volatile("" :: "r"(warm));
 #endif
                 if ((V & 1) == 0) run_batch_copies<W>(dst, s.lits, nb, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
-                else run_batch_copies_pool<W>(dst, s.lits, nb, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                else run_batch_copies_pool<W, kDict>(dst, s.lits, nb, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc, dw);
                 c.fp += nb; c.lp += (long)tot_adv + (long)tot_ext; c.op += (long)tot_out;
                 continue;
             }
         }
         LZB_COUNT_SLOW(W::lane() == 0 ? nb : 0);
-        const int e = lz4_serial<W, kPartial>(s, dst, oend, c, nb, oexit);
+        const int e = lz4_serial<W, kPartial, kDict>(s, dst, oend, c, nb, oexit, dw);
         if (e < 0) return e;
         if (kPartial && e > 0) return (int)(c.op - (long)op0);
     }
@@ -1247,10 +1325,13 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lz4(const Strea
 // LIZv1 codewords (lib/lizard_decompress_liz.h:14-220)
 // kPartial: the loop of Lizard_decompress_safe_partial, which returns in front of the first token that starts at or behind
 // `oexit` (op0 + the target); once the flags run out, the block's last literals are copied whatever the target.
-template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lizv1(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh,
-                                                                     long oexit)
+// kDict: as decode_tokens_lz4.
+template <class W, int V, bool kPartial, bool kDict = false>
+LZ_HD int decode_tokens_lizv1(const Streams& s, u8* dst, u32 op0, u32 oend_u, DecWarpShared* sh, long oexit, DictWin dw = DictWin())
 {
+    static_assert(!kDict || (V & 1) != 0, "dictionary matches need the pooled copy sweeps");
     const long nl = (long)s.nlits, oend = (long)oend_u;
+    const long reach = kDict ? (long)dw.reach : 0;
     const u32 NL = W::lanes(), lane = W::lane();
     if (oend_u - op0 == 0) return (s.nflags == 1 && s.flags[0] == 0) ? 0 : -1;
     TokCursor c; c.fp = 0; c.lp = 0; c.op = op0; c.p16 = c.p24 = 0; c.last_off = 0;
@@ -1360,7 +1441,7 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lizv1(const Str
             const long opos = c.op + (long)O;
             if (act && !bad) {
                 if (shortf && opos + (long)lit_len > oend - 16) bad = true;
-                else if ((long)off > opos + (long)lit_len) bad = true;
+                else if ((long)off > opos + (long)lit_len + reach) bad = true;
                 else if (opos + (long)lit_len + (long)ml > oend - 16) bad = true;
             }
             if (kPartial) {
@@ -1374,7 +1455,7 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lizv1(const Str
                         const u32 end = W::shfl(O, e);
                         if (e > 0) {
                             if ((V & 1) == 0) run_batch_copies<W>(dst, s.lits, e, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
-                            else run_batch_copies_pool<W>(dst, s.lits, e, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                            else run_batch_copies_pool<W, kDict>(dst, s.lits, e, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc, dw);
                             W::sync();
                         }
                         return (int)(c.op + (long)end - (long)op0);
@@ -1385,7 +1466,7 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lizv1(const Str
                 LZB_COUNT_FAST(W::lane() == 0 ? nb : 0);
                 if (LZB_DEC_LIT_PF_NEXT) { const long nx = c.lp + (long)tot_adv + (long)tot_ext + 128 * (long)lane; if (lane < LZB_DEC_LIT_PF_LINES && nx < nl) W::prefetch(s.lits + nx); }
                 if ((V & 1) == 0) run_batch_copies<W>(dst, s.lits, nb, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
-                else run_batch_copies_pool<W>(dst, s.lits, nb, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc);
+                else run_batch_copies_pool<W, kDict>(dst, s.lits, nb, (u32)lit_src, lit_len, (u32)opos, off, ml, sh->desc, dw);
                 c.fp += nb; c.lp += (long)tot_adv + (long)tot_ext; c.op += (long)tot_out;
                 c.p16 += tot16; c.p24 += tot24;
                 c.last_off = W::shfl(off, nb - 1);
@@ -1393,7 +1474,7 @@ template <class W, int V, bool kPartial> LZ_HD int decode_tokens_lizv1(const Str
             }
         }
         LZB_COUNT_SLOW(W::lane() == 0 ? nb : 0);
-        const int e = lizv1_serial<W, kPartial>(s, dst, oend, c, nb, oexit);
+        const int e = lizv1_serial<W, kPartial, kDict>(s, dst, oend, c, nb, oexit, dw);
         if (e < 0) return e;
         if (kPartial && e > 0) return (int)(c.op - (long)op0);
     }
@@ -1458,10 +1539,12 @@ template <class W> LZ_HD int read_stream(bool huff, const u8* src, long csize, l
 // kPartial: Lizard_decompress_safe_partial with targetOutputSize = `target` (lib/lizard_decompress.c:272-275).  The unit stops
 // after the inner block that brings its output to `target` or beyond (:175 for a raw block, :249), and each block's token
 // loop stops at its own start + `target`.  Nothing behind the stopping point is read.  Partial units never use the pre-passes.
-template <class W, int V, bool kPartial = false>
+// kDict: Lizard_decompress_safe_usingDict with the dictionary `dw` (its reach 0: none).  The Huffman pre-pass may have expanded
+// the streams (`up`); the token pre-pass, which checks offsets against the unit start, is never used.
+template <class W, int V, bool kPartial = false, bool kDict = false>
 LZ_HD int decode_unit(const u8* src, u32 csize_u, u8* dst, u32 cap, u8* scratch, DecWarpShared* sh,
                       const UnitPre* up = nullptr, const u8* arena = nullptr,
-                      const UnitSeq* us = nullptr, const PoolRun* recs = nullptr, int target = 0)
+                      const UnitSeq* us = nullptr, const PoolRun* recs = nullptr, int target = 0, DictWin dw = DictWin())
 {
     const long csize = (long)csize_u;
     if (csize < 1) return 0;
@@ -1504,9 +1587,9 @@ LZ_HD int decode_unit(const u8* src, u32 csize_u, u8* dst, u32 cap, u8* scratch,
         if (!read_stream<W>(hdr & kFlagLiterals, src, csize, ip, scratch, &s.lits, &s.nlits, sh, pre_lits)) return -1;
         if (ip > csize) return -1;
         int res;
-        if (!kPartial && us != nullptr && ip0 == 1 && us->state == kPreDone) res = decode_block_from_records<W>(s, dst, (u32)op, us, recs, sh);
-        else res = lizv1 ? decode_tokens_lizv1<W, V, kPartial>(s, dst, (u32)op, cap, sh, op + target)
-                         : decode_tokens_lz4<W, V, kPartial>(s, dst, (u32)op, cap, sh, op + target);
+        if (!kPartial && !kDict && us != nullptr && ip0 == 1 && us->state == kPreDone) res = decode_block_from_records<W>(s, dst, (u32)op, us, recs, sh);
+        else res = lizv1 ? decode_tokens_lizv1<W, V, kPartial, kDict>(s, dst, (u32)op, cap, sh, op + target, dw)
+                         : decode_tokens_lz4<W, V, kPartial, kDict>(s, dst, (u32)op, cap, sh, op + target, dw);
         if (res <= 0) return res;
         op += res;
         if (kPartial && op >= (long)target) break;

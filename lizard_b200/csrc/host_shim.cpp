@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #define LZB_SHIM_CHECK(cond) do { if (!(cond)) { fprintf(stderr, "host shim check failed: %s (%s:%d)\n", #cond, __FILE__, __LINE__); abort(); } } while (0)
+#define LZB_DICT_STATS 1          /* count the dictionary decoder's matches (lzb_dict_stats) */
 #include "entropy_dec.cuh"
 #include "encode_core.cuh"
 #include "decode.cuh"
@@ -92,6 +93,31 @@ extern "C" int lzb_host_decompress_partial(const unsigned char* src, int csize, 
                                                             nullptr, nullptr, nullptr, nullptr, target);
     free(scratch); free(sh);
     return r;
+}
+
+// Lizard_decompress_safe_usingDict through the one-lane instantiation of the dictionary decoder (the device's dictionary
+// kernel without the Huffman pre-pass): the `avail` bytes in front of dict_end are the dictionary, `reach` how far below the
+// unit start a match may start (dict_reach; 0xffffffff = unchecked)
+extern "C" int lzb_host_decompress_dict(const unsigned char* src, int csize, unsigned char* dst, int cap,
+                                        const unsigned char* dict_end, unsigned avail, unsigned reach)
+{
+    if (csize < 1) return 0;
+    if (cap < 0) return -1;
+    unsigned char* scratch = (unsigned char*)malloc(lzb::kDecScratchPerWarp);
+    lzb::DecWarpShared* sh = (lzb::DecWarpShared*)malloc(sizeof(lzb::DecWarpShared));
+    sh->big_table = (lzb::u16*)(scratch + 4 * lzb::kDecStreamScratch);
+    lzb::DictWin dw; dw.end = dict_end; dw.avail = avail; dw.reach = reach;
+    const int r = lzb::decode_unit<lzb::HostLanes, 3, false, true>(src, (lzb::u32)csize, dst, (lzb::u32)cap, scratch, sh,
+                                                                   nullptr, nullptr, nullptr, nullptr, 0, dw);
+    free(scratch); free(sh);
+    return r;
+}
+
+// matches the dictionary decoders above and below have read from the dictionary alone / across its end since the last reset
+extern "C" void lzb_dict_stats(unsigned long long* only, unsigned long long* straddle, int reset)
+{
+    *only = lzb::g_dict_only; *straddle = lzb::g_dict_straddle;
+    if (reset) lzb::g_dict_only = lzb::g_dict_straddle = 0;
 }
 
 // The Huffman pre-pass (huf_expand.cuh) as the device runs it, serially: plan the unit's first inner block, expand the
@@ -365,6 +391,34 @@ extern "C" int lzb_emu_decompress_partial(const unsigned char* src, int csize, u
     a.sh = (lzb::DecWarpShared*)malloc(sizeof(lzb::DecWarpShared));
     a.sh->big_table = (lzb::u16*)(a.scratch + 4 * lzb::kDecStreamScratch);
     emu::run(emu_partial_body, &a);
+    free(a.scratch); free(a.sh);
+    return a.result;
+}
+
+struct EmuDictArgs { const unsigned char* src; int csize; unsigned char* dst; int cap; lzb::DictWin dw; unsigned char* scratch;
+                     lzb::DecWarpShared* sh; int result; };
+static void emu_dict_body(void* p)
+{
+    EmuDictArgs* a = (EmuDictArgs*)p;
+    const int r = lzb::decode_unit<EmuLanes, 3, false, true>(a->src, (lzb::u32)a->csize, a->dst, (lzb::u32)a->cap, a->scratch, a->sh,
+                                                             nullptr, nullptr, nullptr, nullptr, 0, a->dw);
+    if (EmuLanes::lane() == 0) a->result = r;
+}
+
+// Lizard_decompress_safe_usingDict through the 32-lane emulation of the device's dictionary kernel (arguments as
+// lzb_host_decompress_dict)
+extern "C" int lzb_emu_decompress_dict(const unsigned char* src, int csize, unsigned char* dst, int cap,
+                                       const unsigned char* dict_end, unsigned avail, unsigned reach)
+{
+    if (csize < 1) return 0;
+    if (cap < 0) return -1;
+    EmuDictArgs a;
+    a.src = src; a.csize = csize; a.dst = dst; a.cap = cap; a.result = -1;
+    a.dw.end = dict_end; a.dw.avail = avail; a.dw.reach = reach;
+    a.scratch = (unsigned char*)malloc(lzb::kDecScratchPerWarp);
+    a.sh = (lzb::DecWarpShared*)malloc(sizeof(lzb::DecWarpShared));
+    a.sh->big_table = (lzb::u16*)(a.scratch + 4 * lzb::kDecStreamScratch);
+    emu::run(emu_dict_body, &a);
     free(a.scratch); free(a.sh);
     return a.result;
 }
