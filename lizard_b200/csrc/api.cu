@@ -5,6 +5,7 @@
 #include "decode2.cuh"
 #include "prepass.cuh"
 #include "encode.cuh"
+#include "encode_lp_kernel.cuh"
 
 #include <cuda_runtime.h>
 #include <mutex>
@@ -544,13 +545,15 @@ int launch_decode_dict(Context& c, const void* dSrc, const u64* dSrcOff, const u
     return LIZARDB200_OK;
 }
 
+// levels the encoder implements: the parsers of level_params(), and lowestPrice (23-25, 43-45) in a kernel of its own
+bool enc_level_ok(int level) { return level_params(level).parser != kParserUnsupported || lp_level(level); }
+
 int launch_encode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* dSrcLen,
                   void* dDst, const u64* dDstOff, const u32* dDstCap, int* dResult, u32 n, int level, cudaStream_t s,
-                  const Progress* pg = nullptr, const FramePack* fp = nullptr)
+                  const Progress* pg = nullptr, const FramePack* fp = nullptr, bool big_units = true)
 {
     if (n == 0) return LIZARDB200_OK;
-    LevelParams lp = level_params(level);
-    if (lp.parser == kParserUnsupported) { g_last_error = "compression level not implemented on the GPU"; return LIZARDB200_ERR_LEVEL; }
+    if (!enc_level_ok(level)) { g_last_error = "compression level not implemented on the GPU"; return LIZARDB200_ERR_LEVEL; }
     workspace_acquire(c, s);
     struct Release { Context& c; cudaStream_t s; ~Release() { workspace_release(c, s); } } release_on_exit{c, s};
     EncodeBatch b;
@@ -562,7 +565,7 @@ int launch_encode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* d
     b.scratch = (u8*)c.enc_scratch.p;
     b.counter = next_counter(c, s);
     int launches = 0;
-    cudaError_t e = encode_launch(c.enc_cfg, b, s, &launches);
+    cudaError_t e = lp_level(level) ? lp_encode_launch(c.enc_cfg, b, s, &launches, big_units) : encode_launch(c.enc_cfg, b, s, &launches);
     g_launches += (unsigned long long)launches;
     if (e != cudaSuccess) { fail("encode launch", e); return LIZARDB200_ERR_CUDA; }
     return LIZARDB200_OK;
@@ -586,7 +589,7 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
     std::lock_guard<std::mutex> lock(c.mu);
     int st = ensure_context(c, g_device);
     if (st != LIZARDB200_OK) return st;
-    if (kCompress && level_params(level).parser == kParserUnsupported) {
+    if (kCompress && !enc_level_ok(level)) {
         g_last_error = "compression level not implemented on the GPU";
         return LIZARDB200_ERR_LEVEL;
     }
@@ -666,7 +669,11 @@ int run_host_batch(const void* const* src, const int* srcSize, void* const* dst,
     const u32* d_dict_reach = d_dict_len + nd;
     const int* d_target = (const int*)(d_dict_reach + nd);
     int* d_res = (int*)d_target + (target ? n : 0);
-    if (kCompress) st = launch_encode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, level, s);
+    if (kCompress) {
+        bool big = false;                                         // a unit of several inner blocks (lowestPrice big slots)
+        for (int i = 0; i < n; ++i) big = big || (u32)srcSize[i] > kBlockSize;
+        st = launch_encode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, level, s, nullptr, nullptr, big);
+    }
     else if (target) st = launch_decode_partial(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_target, d_res, (u32)n, s);
     else if (dict) st = launch_decode_dict(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, c.d_in.p, d_dict_off,
                                            d_dict_len, d_dict_reach, d_res, (u32)n, s);
@@ -728,6 +735,14 @@ unsigned long long LizardB200_launchCount(void) { return g_launches.load(); }
 // device): warps per CTA, how many of them keep their hash table in shared memory, CTAs per SM, dynamic shared bytes per CTA
 int LizardB200_encodeShape(int level, int* warpsPerCta, int* smemTables, int* ctasPerSM, int* smemBytes)
 {
+    if (lp_level(level)) {          // the lowestPrice kernel: no shared-memory tables, 16 KiB of static histograms per CTA
+        const LpShape sh = lp_shape();
+        if (warpsPerCta) *warpsPerCta = sh.warps;
+        if (smemTables) *smemTables = 0;
+        if (ctasPerSM) *ctasPerSM = sh.ctas_per_sm;
+        if (smemBytes) *smemBytes = 0;
+        return LIZARDB200_OK;
+    }
     const LevelParams lp = level_params(level);
     if (lp.parser == kParserUnsupported) return LIZARDB200_ERR_LEVEL;
     const EncodeShape sh = encode_shape_in_effect(lp);
@@ -849,7 +864,7 @@ int LizardB200_compress_blocks(const void* src, size_t srcSize, int blockSize,
     std::lock_guard<std::mutex> lock(c.mu);
     int st = ensure_context(c, g_device);
     if (st != LIZARDB200_OK) return st;
-    if (level_params(level).parser == kParserUnsupported) { g_last_error = "compression level not implemented on the GPU"; return LIZARDB200_ERR_LEVEL; }
+    if (!enc_level_ok(level)) { g_last_error = "compression level not implemented on the GPU"; return LIZARDB200_ERR_LEVEL; }
     const size_t tab_bytes = n * (8 + 4 + 8 + 4 + 4);
     CU_OK(c.pin_tab.reserve(tab_bytes));
     CU_OK(c.d_tab.reserve(tab_bytes));
@@ -872,7 +887,8 @@ int LizardB200_compress_blocks(const void* src, size_t srcSize, int blockSize,
     CU_OK(cudaMemcpyAsync(dtab, c.pin_tab.p, tab_bytes - n * 4, cudaMemcpyHostToDevice, s));
     const u64* d_in_off = (const u64*)dtab; const u64* d_out_off = d_in_off + n;
     const u32* d_in_len = (const u32*)(d_out_off + n); const u32* d_out_cap = d_in_len + n; int* d_res = (int*)(d_out_cap + n);
-    st = launch_encode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, level, s);
+    st = launch_encode(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, d_res, (u32)n, level, s, nullptr, nullptr,
+                       (size_t)blockSize > kBlockSize);
     if (st != LIZARDB200_OK) return st;
     CU_OK(cudaMemcpyAsync(t_res, d_res, n * 4, cudaMemcpyDeviceToHost, s));
     CU_OK(cudaMemcpyAsync(dst, c.d_out.p, n * dstStride, cudaMemcpyDeviceToHost, s));

@@ -7,8 +7,10 @@
 #include <stdlib.h>
 #define LZB_SHIM_CHECK(cond) do { if (!(cond)) { fprintf(stderr, "host shim check failed: %s (%s:%d)\n", #cond, __FILE__, __LINE__); abort(); } } while (0)
 #define LZB_DICT_STATS 1          /* count the dictionary decoder's matches (lzb_dict_stats) */
+#define LZB_LP_STATS 1            /* count the lowestPrice parser's rare paths (lzb_lp_stats) */
 #include "entropy_dec.cuh"
 #include "encode_core.cuh"
+#include "encode_lp.cuh"
 #include "decode.cuh"
 #include "decode2.cuh"
 #include <stdlib.h>
@@ -41,11 +43,42 @@ static lzb::HashTable make_table(lzb::u32* buf, int n, const lzb::LevelParams& l
     return T;
 }
 
+unsigned long long lzb::g_lp_stats[lzb::kLpStats];
+extern "C" void lzb_lp_stats(unsigned long long* out, int reset)
+{
+    for (int k = 0; k < lzb::kLpStats; ++k) { if (out) out[k] = lzb::g_lp_stats[k]; if (reset) lzb::g_lp_stats[k] = 0; }
+}
+
+// the lowestPrice levels' scratch as the device kernel sets it up: a zero map (epoch 1), and for units of several inner
+// blocks a zero big slot
+struct LpScratch {
+    lzb::LpWork* work; lzb::u8* big;
+    explicit LpScratch(int n)
+    {
+        work = (lzb::LpWork*)malloc(sizeof(lzb::LpWork));
+        memset(work->map, 0, sizeof work->map);
+        work->huf.seg_count = (lzb::u32 (*)[256])malloc(4 * 256 * sizeof(lzb::u32));
+        big = (lzb::u32)n > lzb::kBlockSize ? (lzb::u8*)calloc(1, lzb::kLpBigSlotBytes) : nullptr;
+    }
+    ~LpScratch()
+    {
+        if (big) {   // the unit must leave its table zero for the next holder of the slot
+            const lzb::u32* t = (const lzb::u32*)big;
+            for (size_t i = 0; i < lzb::kLpBigTableBytes / 4; ++i) LZB_SHIM_CHECK(t[i] == 0);
+        }
+        free(work->huf.seg_count); free(work); free(big);
+    }
+};
+
 extern "C" int lzb_host_compress(const unsigned char* src, int n, unsigned char* dst, int cap, int level)
 {
     if (n < 0 || cap < 0) return 0;
     if (level > 49) level = 49;
     if (level < 10) level = 17;
+    if (lzb::lp_level(level)) {
+        LpScratch sc(n);
+        return lzb::encode_unit_lp<lzb::HostLanes>(src, (lzb::u32)n, dst, (lzb::u32)cap, level, sc.work, 1, sc.big);
+    }
     lzb::LevelParams lp = lzb::level_params(level);
     if (lp.parser == lzb::kParserUnsupported) return 0;
     lzb::u32* table = (lzb::u32*)malloc(sizeof(lzb::u32) << lp.hashLog);
@@ -321,12 +354,26 @@ static void emu_compress_body(void* p)
     if (EmuLanes::lane() == 0) a->result = r;
 }
 
+struct EmuLpArgs { const unsigned char* src; int n; unsigned char* dst; int cap; int level; LpScratch* sc; int result; };
+static void emu_lp_body(void* p)
+{
+    EmuLpArgs* a = (EmuLpArgs*)p;
+    int r = lzb::encode_unit_lp<EmuLanes>(a->src, (lzb::u32)a->n, a->dst, (lzb::u32)a->cap, a->level, a->sc->work, 1, a->sc->big);
+    if (EmuLanes::lane() == 0) a->result = r;
+}
+
 // Lizard_compress through the 32-lane emulation of the device code path
 extern "C" int lzb_emu_compress(const unsigned char* src, int n, unsigned char* dst, int cap, int level)
 {
     if (n < 0 || cap < 0) return 0;
     if (level > 49) level = 49;
     if (level < 10) level = 17;
+    if (lzb::lp_level(level)) {
+        LpScratch sc(n);
+        EmuLpArgs a = { src, n, dst, cap, level, &sc, 0 };
+        emu::run(emu_lp_body, &a);
+        return a.result;
+    }
     lzb::LevelParams lp = lzb::level_params(level);
     if (lp.parser == lzb::kParserUnsupported) return 0;
     EmuCompressArgs a;
