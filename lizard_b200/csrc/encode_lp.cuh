@@ -97,12 +97,30 @@ LZ_HD bool lp_more_profitable(u32 best_off, u64 best_common, u32 off, u64 common
 // delta clamped to maxDistance, which ends the walk at the lowLimit test).  Positions are chain[pos & mask]: the bias 2^24
 // is a multiple of 2^22, so `index & contentMask` is the position modulo 2^22, and a unit of one inner block needs 2^17.
 enum : u32 { kLpMapLog = 18, kLpEpochMax = (1u << 23) - 1 };
+#if defined(LZB_LP_STATS) && !defined(__CUDA_ARCH__)
+// host shim only: every slot a lookup or insert visits past its home slot (tests prove that hostile input builds long
+// probe runs and runs that wrap past the last slot)
+enum { kLpProbeLongest, kLpProbes, kLpProbeWraps, kLpProbeStats };
+extern unsigned long long g_lp_probe[kLpProbeStats];
+inline void lp_probe_count(u32 home, u32 i)
+{
+    if (i == home) return;
+    const unsigned long long run = (i - home) & ((1u << kLpMapLog) - 1);
+    g_lp_probe[kLpProbes]++;
+    if (run > g_lp_probe[kLpProbeLongest]) g_lp_probe[kLpProbeLongest] = run;
+    if (i == 0) g_lp_probe[kLpProbeWraps]++;
+}
+#define LZB_LP_PROBE(home, i) lp_probe_count(home, i)
+#else
+#define LZB_LP_PROBE(home, i) do { } while (0)
+#endif
 struct LpMap {
     u64* slot; u64 tag; u32 shift;
     LZ_HDM LpMap(u64* s, u32 epoch, u32 hash_log) : slot(s), tag((u64)epoch << 41), shift(hash_log - kLpMapLog) {}
     LZ_HDM u32 get(u32 h) const
     {
         for (u32 i = h >> shift;; i = (i + 1) & ((1u << kLpMapLog) - 1)) {
+            LZB_LP_PROBE(h >> shift, i);
             const u64 e = slot[i];
             if ((e & ~((1ull << 41) - 1)) != tag) return 0;
             if ((u32)(e >> 18 & 0x7FFFFFu) == h) return (u32)(e & 0x3FFFFu) - 1 + kDictSize;
@@ -112,6 +130,7 @@ struct LpMap {
     {
         const u64 v = tag | (u64)h << 18 | (u64)(abs_index - kDictSize + 1);
         for (u32 i = h >> shift;; i = (i + 1) & ((1u << kLpMapLog) - 1)) {
+            LZB_LP_PROBE(h >> shift, i);
             const u64 e = slot[i];
             if ((e & ~((1ull << 41) - 1)) != tag) {            // empty: claim it (lanes of other buckets may race for it)
 #if defined(__CUDA_ARCH__)

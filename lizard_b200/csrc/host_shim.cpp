@@ -3,6 +3,7 @@
 // __host__ __device__ code (entropy_dec.cuh / entropy_enc.cuh / encode_core.cuh, instantiated with the
 // one-lane policy HostLanes) against the reference library without a GPU.  Nothing in the product
 // path links or loads this file; liblizard_b200.so has no CPU code path.
+#include <stddef.h>
 #include <stdio.h>
 #include <stdlib.h>
 #define LZB_SHIM_CHECK(cond) do { if (!(cond)) { fprintf(stderr, "host shim check failed: %s (%s:%d)\n", #cond, __FILE__, __LINE__); abort(); } } while (0)
@@ -385,6 +386,107 @@ extern "C" int lzb_emu_compress(const unsigned char* src, int n, unsigned char* 
     emu::run(emu_compress_body, &a);
     free(a.work->huf.seg_count); free(table); free(a.work);
     return a.result;
+}
+
+// ---- lowestPrice on persistent, poisoned scratch ------------------------------------------------------------------------
+// A device warp does not get clean scratch per unit: its LpWork keeps whatever the previous unit (of this launch, or of
+// another encoder that shares the workspace) left, its map holds entries of earlier epochs, and a big slot's chain is
+// never cleared.  These entry points keep one such scratch across calls, so the tests can run sequences of units on it.
+struct LpPersist { lzb::LpWork* work; lzb::u8* big; lzb::u32 (*seg)[256]; };
+static lzb::u32 lp_rand(lzb::u32& s) { s = s * 1664525u + 1013904223u; return s ^ (s >> 15); }
+static void lp_fill(void* p, size_t n, lzb::u32 seed)
+{
+    lzb::u32* w = (lzb::u32*)p;
+    for (size_t i = 0; i < n / 4; ++i) w[i] = lp_rand(seed);
+}
+// garbage in the sequence list, chain, streams and Huffman scratch; a big slot whose table is zero and whose chain is garbage
+extern "C" void* lzb_lp_scratch_new(unsigned seed)
+{
+    LpPersist* sc = (LpPersist*)malloc(sizeof(LpPersist));
+    sc->work = (lzb::LpWork*)malloc(sizeof(lzb::LpWork));
+    sc->seg = (lzb::u32 (*)[256])malloc(4 * 256 * sizeof(lzb::u32));
+    lp_fill(sc->work, offsetof(lzb::LpWork, map), seed);
+    lp_fill(sc->seg, 4 * 256 * sizeof(lzb::u32), seed + 1);
+    sc->work->huf.seg_count = sc->seg;
+    memset(sc->work->map, 0, sizeof sc->work->map);
+    sc->big = (lzb::u8*)calloc(1, lzb::kLpBigSlotBytes);
+    lp_fill(sc->big + lzb::kLpBigTableBytes, lzb::kLpBigChainBytes, seed + 2);
+    return sc;
+}
+extern "C" void lzb_lp_scratch_free(void* p)
+{
+    LpPersist* sc = (LpPersist*)p;
+    free(sc->seg); free(sc->work); free(sc->big); free(sc);
+}
+// A map as a warp may find it before a unit at `epoch`, filled with entries of other epochs (0, epoch - 1, epoch + 1 and
+// kLpEpochMax, in turn):
+//  * every slot holds a stale bucket whose home it is (at `hash_log`), with a random position;
+//  * with `src`, the stale entries of the next unit's own buckets, placed where the map's probing would find them: for each
+//    position p that the unit inserts, bucket(p) -> p - k (k = 1..7).  Taken for a current entry, such an entry lies within
+//    8 bytes below p, so Lizard_Insert's "replace unless within 8" rule keeps it instead of p, and the parse loses matches.
+// A map that counts every slot of another epoch as empty gives the unit the reference's bytes.
+extern "C" void lzb_lp_scratch_poison_map(void* p, unsigned epoch, unsigned hash_log, unsigned seed,
+                                          const unsigned char* src, int n, unsigned mls)
+{
+    LpPersist* sc = (LpPersist*)p;
+    lzb::u64* const map = sc->work->map;
+    const lzb::u32 shift = hash_log - lzb::kLpMapLog, mx = lzb::kLpEpochMax, mask = (1u << lzb::kLpMapLog) - 1;
+    lzb::u32 other[4] = { 0u, (epoch - 1) & mx, (epoch + 1) & mx, mx };
+    for (lzb::u32& e : other)
+        if (e == epoch) e = (epoch + 2) & mx;          // epoch 1: epoch - 1 is 0; kLpEpochMax: epoch + 1 wraps to 0
+    for (lzb::u32 i = 0; i <= mask; ++i) {
+        const lzb::u32 bucket = (i << shift) | (lp_rand(seed) & ((1u << shift) - 1));
+        const lzb::u32 pos1 = 1 + lp_rand(seed) % lzb::kBlockSize;
+        map[i] = (lzb::u64)other[i & 3] << 41 | (lzb::u64)bucket << 18 | pos1;
+    }
+    if (!src || n <= (int)lzb::kMfLimit) return;
+    std::vector<unsigned char> placed(mask + 1, 0);
+    for (lzb::u32 q = 1; q < (lzb::u32)n - lzb::kMfLimit && q < lzb::kBlockSize; ++q) {
+        const lzb::u32 h = lzb::hc_hash(src + q, hash_log, mls);
+        lzb::u32 i = h >> shift;
+        bool dup = false;
+        for (; placed[i]; i = (i + 1) & mask)
+            if ((lzb::u32)(map[i] >> 18 & 0x7FFFFFu) == h) { dup = true; break; }
+        if (dup) continue;
+        const lzb::u32 k = 1 + lp_rand(seed) % 7, stale = q > k ? q - k : 0;
+        map[i] = (lzb::u64)other[q & 3] << 41 | (lzb::u64)h << 18 | (stale + 1);
+        placed[i] = 1;
+    }
+}
+// the kernel's rule when a warp's epoch reaches kLpEpochMax: clear the map, go on at epoch 1
+extern "C" void lzb_lp_scratch_clear_map(void* p) { memset(((LpPersist*)p)->work->map, 0, sizeof ((LpPersist*)p)->work->map); }
+// 1 if the big slot's table is zero, as every unit must leave it
+extern "C" int lzb_lp_scratch_big_clean(void* p)
+{
+    const lzb::u32* t = (const lzb::u32*)((LpPersist*)p)->big;
+    for (size_t i = 0; i < lzb::kLpBigTableBytes / 4; ++i) if (t[i]) return 0;
+    return 1;
+}
+
+struct EmuLpOnArgs { const unsigned char* src; int n; unsigned char* dst; int cap; int level; LpPersist* sc; unsigned epoch; int result; };
+static void emu_lp_on_body(void* p)
+{
+    EmuLpOnArgs* a = (EmuLpOnArgs*)p;
+    int r = lzb::encode_unit_lp<EmuLanes>(a->src, (lzb::u32)a->n, a->dst, (lzb::u32)a->cap, a->level, a->sc->work, a->epoch, a->sc->big);
+    if (EmuLanes::lane() == 0) a->result = r;
+}
+// one unit at a lowestPrice level on the persistent scratch under `epoch` (1 .. kLpEpochMax); emu = 32 emulated lanes
+extern "C" int lzb_lp_compress_on(void* p, const unsigned char* src, int n, unsigned char* dst, int cap, int level,
+                                  unsigned epoch, int emu)
+{
+    LpPersist* sc = (LpPersist*)p;
+    if (n < 0 || cap < 0 || !lzb::lp_level(level) || epoch < 1 || epoch > lzb::kLpEpochMax) return 0;
+    if (!emu) return lzb::encode_unit_lp<lzb::HostLanes>(src, (lzb::u32)n, dst, (lzb::u32)cap, level, sc->work, epoch, sc->big);
+    EmuLpOnArgs a = { src, n, dst, cap, level, sc, epoch, 0 };
+    emu::run(emu_lp_on_body, &a);
+    return a.result;
+}
+
+unsigned long long lzb::g_lp_probe[lzb::kLpProbeStats];
+// longest probe run, slots probed past the home slot, probes that wrapped past the map's last slot
+extern "C" void lzb_lp_probe_stats(unsigned long long* out, int reset)
+{
+    for (int k = 0; k < lzb::kLpProbeStats; ++k) { if (out) out[k] = lzb::g_lp_probe[k]; if (reset) lzb::g_lp_probe[k] = 0; }
 }
 
 struct EmuDecompressArgs { const unsigned char* src; int csize; unsigned char* dst; int cap; unsigned char* scratch; lzb::DecWarpShared* sh; int result;

@@ -235,6 +235,129 @@ def corpus():
     return {"far": far_units(), "threshold": threshold_units(), "hostile": hostile_units(), "periodic": periodic_units()}
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# collide: inputs built against the lowestPrice map (csrc/encode_lp.cuh, LpMap)
+# ---------------------------------------------------------------------------------------------------------------------
+# The lowestPrice levels hash a position's 4 bytes (Lizard_hashPtr, searchLength 4: level 25/45) or 5 bytes (Lizard_hash5:
+# 23/24/43/44) to a bucket of hashLog bits.  A unit of one inner block keeps (bucket, position) pairs in a map of 2^18
+# slots whose home slot is the bucket's top 18 bits, probed linearly, so at hashLog 23 (24/25/44/45) 32 buckets share a
+# home slot.  Both hashes are invertible (odd multipliers), so keys of any chosen bucket can be written down.
+MAP_LOG = 18
+HASH4_PRIME, HASH5_PRIME = 2654435761, 889523592379
+_INV4, _INV5 = pow(HASH4_PRIME, -1, 1 << 32), pow(HASH5_PRIME, -1, 1 << 40)
+
+
+def bucket(window: bytes, hash_log: int) -> int:
+    """hc_hash of a 4-byte (searchLength 4) or 5-byte window."""
+    if len(window) == 4:
+        return (int.from_bytes(window, "little") * HASH4_PRIME % (1 << 32)) >> (32 - hash_log)
+    return (int.from_bytes(window, "little") * HASH5_PRIME % (1 << 40)) >> (40 - hash_log)
+
+
+def key(b: int, mls: int, rnd, hash_log=23) -> bytes:
+    """`mls` bytes (4 or 5) whose bucket at `hash_log` is b; the low bits of the product are random."""
+    bits = 32 if mls == 4 else 40
+    low = bits - hash_log
+    x = (b << low) | rnd.getrandbits(low)
+    v = x * (_INV4 if mls == 4 else _INV5) % (1 << bits)
+    return v.to_bytes(mls, "little")
+
+
+def collide_unit(seed, mls, first, keys=2048, n=BS, background="random", repeat=False):
+    """A unit of `n` bytes with `keys` planted keys of consecutive hashLog-23 buckets first, first + 1, ..., one at the start
+    of each 8-byte record from n // 8 on.  The keys are inserted in bucket order, so each one probes past the slots of the
+    keys before it that share or precede its home slot: long probe runs, and with `first` near 2^23 runs that wrap past the
+    map's last slot.  repeat=True follows every record with a copy of an earlier record (key and 3 bytes), so the parser
+    finds matches of 7 bytes through the runs."""
+    rnd = random.Random(seed)
+    rng = np.random.default_rng(seed)
+    out = bytearray(_random(rng, n) if background == "random" else lz.datagen(n, 50, seed))
+    step = 16 if repeat else 8
+    at = max(0, min(n // 8, n - keys * step - 64))
+    assert at + keys * step + 64 <= n
+    recs = []
+    for i in range(keys):
+        r = key(first + i, mls, rnd) + bytes(rnd.getrandbits(8) for _ in range(8 - mls))
+        out[at + step * i:at + step * i + 8] = r
+        recs.append(r)
+        if repeat:
+            j = rnd.randrange(i + 1)
+            out[at + step * i + 8:at + step * i + 16] = recs[j][:7] + bytes([recs[j][7] ^ 0x5A])
+    return bytes(out[:n])
+
+
+def race_unit(seed, mls, n=BS, pairs=48):
+    """Pairs of new buckets that share a home slot and are inserted by one 32-position insert step, so that two lanes claim
+    the same empty slot at once (on the device, one loses the atomic compare-and-swap and must go on probing).
+
+    A literal-only parse inserts one position per step; only the positions behind a match are inserted many at a time, and
+    of those only the last mls - 1 have windows that did not occur before.  So each pair is a 32-byte match ending at E whose
+    last bytes and the two bytes behind it are chosen: the windows at E - mls + 1 and E - mls + 2 have the same home slot.
+    Copies of each of the two windows alone appear later, each a match of exactly one window, found only if its position
+    was inserted.  A map that drops the insert of the lane that lost the race changes the stream."""
+    rnd = random.Random(seed)
+    rng = np.random.default_rng(seed)
+    hl, bits = 23, 8 * mls
+    prime, mask = (HASH4_PRIME, 0xFFFFFFFF) if mls == 4 else (HASH5_PRIME, (1 << 40) - 1)
+    found = []
+    while len(found) < pairs:
+        # w0 random; w1 = w0's last mls - 1 bytes + one byte t: all 256 t at once
+        w0 = rng.integers(0, 1 << 62, 1 << 14, dtype=np.uint64) & np.uint64(mask)
+        home0 = ((w0 * np.uint64(prime)) & np.uint64(mask)) >> np.uint64(bits - MAP_LOG)
+        w1 = (w0[:, None] >> np.uint64(8)) | (np.arange(256, dtype=np.uint64)[None, :] << np.uint64(bits - 8))
+        home1 = ((w1 * np.uint64(prime)) & np.uint64(mask)) >> np.uint64(bits - MAP_LOG)
+        for r, t in zip(*np.nonzero(home1 == home0[:, None])):
+            a, b = int(w0[r]).to_bytes(mls, "little"), int(w1[r, t]).to_bytes(mls, "little")
+            if bucket(a, hl) != bucket(b, hl):
+                found.append((a, b))
+    found = found[:pairs]
+    # zeros around 8-byte random guards: the block compresses well, so it is not stored raw and its parse shows in the output
+    out = bytearray(n)
+    src_at, copy_at, probe_at = 256, n // 3, 2 * n // 3
+    spans = []
+    for j in range(pairs):
+        spans += [(src_at + 64 * j, 33), (copy_at + 64 * j, 34)]
+        spans += [(probe_at + 64 * j + 24 * k, mls) for k in range(2)]
+    for at, length in spans:
+        out[at - 8:at + length + 8] = _random(rng, length + 16)
+    for j, (a, b) in enumerate(found):
+        body = bytes(_random(rng, 32 - (mls - 1))) + a[:mls - 1]       # the match: 32 bytes ending in w0's first mls - 1
+        s = src_at + 64 * j
+        out[s:s + 32] = body
+        out[s + 32] = a[mls - 1] ^ 0x5A                                 # the source's match ends here
+        c = copy_at + 64 * j
+        out[c - 1] = out[s - 1] ^ 0x33                                  # ... and cannot grow backwards
+        out[c:c + 32] = body
+        out[c + 32:c + 34] = b[mls - 2:]                                # t0, t1
+        e = c + 32                                                      # w0 at e - mls + 1, w1 at e - mls + 2
+        for k, w in enumerate((a, b)):
+            p = probe_at + 64 * j + 24 * k
+            pos = e - mls + 1 + k
+            out[p:p + mls] = w
+            out[p - 1] = out[pos - 1] ^ 0x77
+            out[p + mls] = out[pos + mls] ^ 0x77
+    return bytes(out)
+
+
+def collide_units(seed=80):
+    """The `collide` family, for both key widths: a 2048-key cluster in the middle of the map on random background (a block
+    the encoder stores raw), one straddling the map's end and one whose keys repeat, both on datagen background (their
+    parse shows in the stream), and the insert-race units."""
+    top = (1 << 23) - 2048                              # the last 2048 buckets: the runs of the last home slots wrap
+    out = []
+    for k, mls in enumerate((5, 4)):
+        s = seed + 10 * k
+        out.append(collide_unit(s, mls, 3 << 20))
+        out.append(collide_unit(s + 1, mls, top, background="datagen"))
+        out.append(collide_unit(s + 2, mls, top - 4096, background="datagen", repeat=True))
+        out.append(race_unit(s + 3, mls))
+    return out
+
+
+def corpus_units():
+    return [u for units in corpus().values() for u in units]
+
+
 def edge_capacities(rnd, units, bound):
     """Destination capacities drawn like the GPU edge-input test: the bound twice, one byte short of the input, half of it
     plus one, anything from 1 to the bound."""
@@ -293,7 +416,7 @@ def _copy(out, off, n):
         out += (out[-off:] * (n // off + 1))[:n]
 
 
-def walk(comp):
+def walk(comp, rep_short_at=None):
     """Decode a Lizard stream whose inner blocks carry no Huffman-coded stream (levels 10-29, or blocks of the higher levels
     the encoder stored plain), following Lizard_decompress_generic (lib/lizard_decompress.c:115-264; streams as read by
     Lizard_readStream, :72-112).  Returns (decoded bytes, Counter of codeword classes):
@@ -301,8 +424,10 @@ def walk(comp):
       off16, off24, off_repeat           how a match's offset was coded
       far_short, far_long                LIZv1 24-bit-offset tokens 0-30 and 31
       far_after_literals                 a far token behind a literal-only token (literals before a far match)
+      rep_short                          a repeat-offset match of 2-3 bytes (LIZv1)
       raw_block, block                   stored and coded inner blocks
       ("lit", n), ("match", n), ("far", n)   lengths of literal runs, of 16-bit/repeat matches and of far matches.
+    If `rep_short_at` is a list, the output offset of every rep_short match is appended to it.
     Raises ValueError on a stream the reference would refuse (as far as a valid-stream walker needs to tell)."""
     if not comp:
         raise ValueError("empty input")
@@ -338,7 +463,10 @@ def walk(comp):
             ip += 3 + n
         classes["block"] += 1
         _, off16, off24, flags, lits = (_Stream(s) for s in streams)
-        (_block_liz if lizv1 else _block_lz4)(out, flags, lits, off16, off24, classes)
+        if lizv1:
+            _block_liz(out, flags, lits, off16, off24, classes, rep_short_at)
+        else:
+            _block_lz4(out, flags, lits, off16, off24, classes)
         if lits.p != len(lits.b):                       # last literals: the rest of the stream
             n = len(lits.b) - lits.p
             out += lits.take(n)
@@ -367,7 +495,7 @@ def _block_lz4(out, flags, lits, off16, off24, classes):
         _copy(out, off, ml)
 
 
-def _block_liz(out, flags, lits, off16, off24, classes):
+def _block_liz(out, flags, lits, off16, off24, classes, rep_short_at):
     last_off = 0                                        # LIZARD_INIT_LAST_OFFSET, per inner block
     lit_only = False
     while flags.p < len(flags.b):
@@ -392,6 +520,10 @@ def _block_liz(out, flags, lits, off16, off24, classes):
             else:
                 classes["match_ext0"] += 1
             lit_only = ml == 0
+            if ml and token >> 7 and ml < MINMATCH:       # only lowestPrice writes these: a 2-3 byte repeat-offset match
+                classes["rep_short"] += 1
+                if rep_short_at is not None:
+                    rep_short_at.append(len(out))
             if ml:
                 classes[("match", ml)] += 1
                 _copy(out, last_off, ml)
@@ -416,6 +548,21 @@ def _block_liz(out, flags, lits, off16, off24, classes):
 # ---------------------------------------------------------------------------------------------------------------------
 ENCODE_LEVELS = [10, 11, 13, 14, 15, 16, 17, 20, 21, 22, 30, 31, 34, 35, 36, 37, 38, 40, 41, 42]     # implemented on the GPU
 WALKED_ENCODE_LEVELS = [lv for lv in ENCODE_LEVELS if lv < 30]                                     # no Huffman stage
+# lowestPrice, in a kernel of its own that has one launch shape (LIZARDB200_ENC_SHAPE does not apply)
+LP_ENCODE_LEVELS = [23, 24, 25, 43, 44, 45]
+LP_WALKED_LEVELS = [23, 24, 25]
+
+
+def lp_corpus():
+    """family -> units for the lowestPrice levels: the shared corpus and `collide`."""
+    return dict(corpus(), collide=collide_units())
+
+
+def lp_targets():
+    """Codeword classes the lowestPrice streams of lp_corpus() must contain, summed over its families and LP_WALKED_LEVELS:
+    short repeat matches, 24-bit offsets of both token forms, and every extension width of literal runs and matches."""
+    return ({"rep_short", "off_repeat", "off16", "off24", "far_short", "far_long", "far_after_literals", "raw_block"}
+            | {k + "_ext" + w for k in ("lit", "match") for w in "0134"})
 
 
 def targets(family, lizv1):
