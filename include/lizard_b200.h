@@ -18,8 +18,8 @@
  *      Compression output is byte-identical to the reference built with -DLIZARD_RESET_MEM
  *      (hash table empty at the start of every call), for the levels whose parsers are implemented on
  *      the GPU: 10, 11, 30, 31 (fastSmall / fast), 13-17, 34-38 (hashChain), 20, 40 (fastBig), 21, 22, 41, 42 (priceFast)
- *      and 23-25, 43-45 (lowestPrice).  Any other level (12, 18-19, 26-29, 32-33, 39, 46-49) makes the compress entry
- *      points return 0 ("failed"), never a CPU fallback.
+ *      23-25, 43-45 (lowestPrice) and 18, 19, 39 (the binary-tree optimal parser, LZ4 codewords).  Any other level (12,
+ *      26-29, 32-33, 46-49) makes the compress entry points return 0 ("failed"), never a CPU fallback.
  *      Decompression accepts every level 10..49 (the block format only has two codeword flavours).
  *
  *  (2) BATCH symbols (LizardB200_*): what the reference's per-block loops
@@ -251,7 +251,8 @@ int LizardB200_gather_device(const void* dSrc, const uint64_t* dSrcOff, const in
  * The level's default, or LIZARDB200_ENC_SHAPE="warps,tables,ctas" when that is set and valid, exactly as the encoder
  * launches it.  Levels 23-25 / 43-45 run a kernel of their own with no shared-memory tables (4 warps, 0 tables, 5 CTAs, 0
  * bytes; LIZARDB200_ENC_SHAPE does not apply).  There the encode workspace binds first: on 132 SMs a launch holds 453 CTAs
- * (about 3.4 per SM).  LIZARDB200_ERR_LEVEL for levels whose parser is not implemented. */
+ * (about 3.4 per SM).  Levels 18, 19 and 39 run a kernel of their own with the same shape (4, 0, 5, 0), where the workspace
+ * holds 445 CTAs on 132 SMs.  LIZARDB200_ERR_LEVEL for levels whose parser is not implemented. */
 int LizardB200_encodeShape(int compressionLevel, int* warpsPerCta, int* smemTables, int* ctasPerSM, int* smemBytes);
 /* diagnostics (no device needed): pipeline chunk of a unit in a host-buffer call of nUnits units with unitsPerChunk units per
  * chunk (ramp != 0: the decoder's doubling ramp of small first chunks), computed by the host code and by the kernels'

@@ -6,6 +6,7 @@
 #include "prepass.cuh"
 #include "encode.cuh"
 #include "encode_lp_kernel.cuh"
+#include "encode_opt_kernel.cuh"
 
 #include <cuda_runtime.h>
 #include <mutex>
@@ -545,8 +546,9 @@ int launch_decode_dict(Context& c, const void* dSrc, const u64* dSrcOff, const u
     return LIZARDB200_OK;
 }
 
-// levels the encoder implements: the parsers of level_params(), and lowestPrice (23-25, 43-45) in a kernel of its own
-bool enc_level_ok(int level) { return level_params(level).parser != kParserUnsupported || lp_level(level); }
+// levels the encoder implements: the parsers of level_params(), lowestPrice (23-25, 43-45) and the binary-tree optimal parser
+// with LZ4 codewords (18, 19, 39), each in a kernel of its own
+bool enc_level_ok(int level) { return level_params(level).parser != kParserUnsupported || lp_level(level) || opt_level(level); }
 
 int launch_encode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* dSrcLen,
                   void* dDst, const u64* dDstOff, const u32* dDstCap, int* dResult, u32 n, int level, cudaStream_t s,
@@ -565,7 +567,9 @@ int launch_encode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* d
     b.scratch = (u8*)c.enc_scratch.p;
     b.counter = next_counter(c, s);
     int launches = 0;
-    cudaError_t e = lp_level(level) ? lp_encode_launch(c.enc_cfg, b, s, &launches, big_units) : encode_launch(c.enc_cfg, b, s, &launches);
+    cudaError_t e = lp_level(level) ? lp_encode_launch(c.enc_cfg, b, s, &launches, big_units)
+                  : opt_level(level) ? opt_encode_launch(c.enc_cfg, b, s, &launches, big_units)
+                  : encode_launch(c.enc_cfg, b, s, &launches);
     g_launches += (unsigned long long)launches;
     if (e != cudaSuccess) { fail("encode launch", e); return LIZARDB200_ERR_CUDA; }
     return LIZARDB200_OK;
@@ -735,8 +739,8 @@ unsigned long long LizardB200_launchCount(void) { return g_launches.load(); }
 // device): warps per CTA, how many of them keep their hash table in shared memory, CTAs per SM, dynamic shared bytes per CTA
 int LizardB200_encodeShape(int level, int* warpsPerCta, int* smemTables, int* ctasPerSM, int* smemBytes)
 {
-    if (lp_level(level)) {          // the lowestPrice kernel: no shared-memory tables, 16 KiB of static histograms per CTA
-        const LpShape sh = lp_shape();
+    if (lp_level(level) || opt_level(level)) {   // the lowestPrice / optimal kernels: no shared-memory tables, static histograms
+        const LpShape sh = lp_level(level) ? lp_shape() : opt_shape();
         if (warpsPerCta) *warpsPerCta = sh.warps;
         if (smemTables) *smemTables = 0;
         if (ctasPerSM) *ctasPerSM = sh.ctas_per_sm;

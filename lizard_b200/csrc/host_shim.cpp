@@ -9,9 +9,11 @@
 #define LZB_SHIM_CHECK(cond) do { if (!(cond)) { fprintf(stderr, "host shim check failed: %s (%s:%d)\n", #cond, __FILE__, __LINE__); abort(); } } while (0)
 #define LZB_DICT_STATS 1          /* count the dictionary decoder's matches (lzb_dict_stats) */
 #define LZB_LP_STATS 1            /* count the lowestPrice parser's rare paths (lzb_lp_stats) */
+#define LZB_OPT_STATS 1           /* count the optimal parser's reference behaviours (lzb_opt_stats) */
 #include "entropy_dec.cuh"
 #include "encode_core.cuh"
 #include "encode_lp.cuh"
+#include "encode_opt.cuh"
 #include "decode.cuh"
 #include "decode2.cuh"
 #include <stdlib.h>
@@ -71,6 +73,37 @@ struct LpScratch {
     }
 };
 
+unsigned long long lzb::g_opt_stats[lzb::kOptStats];
+extern "C" void lzb_opt_stats(unsigned long long* out, int reset)
+{
+    for (int k = 0; k < lzb::kOptStats; ++k) { if (out) out[k] = lzb::g_opt_stats[k]; if (reset) lzb::g_opt_stats[k] = 0; }
+}
+
+// the optimal levels' scratch as the device kernel sets it up: a zero map (epoch 1), and for units of several inner blocks a
+// zero big slot; the tree, opt[] and the token statistics start as garbage, as they do on a warp
+struct OptScratch {
+    lzb::OptWork* work; lzb::u8* big; lzb::OptStats* stats;
+    explicit OptScratch(int n)
+    {
+        work = (lzb::OptWork*)malloc(sizeof(lzb::OptWork));
+        memset(work->lp.chain, 0xA5, sizeof work->lp.chain);
+        memset(work->opt, 0x5A, sizeof work->opt);
+        memset(work->lp.map, 0, sizeof work->lp.map);
+        work->lp.huf.seg_count = (lzb::u32 (*)[256])malloc(4 * 256 * sizeof(lzb::u32));
+        stats = (lzb::OptStats*)malloc(sizeof(lzb::OptStats));
+        memset(stats, 0x3C, sizeof *stats);
+        big = (lzb::u32)n > lzb::kBlockSize ? (lzb::u8*)calloc(1, lzb::kLpBigSlotBytes) : nullptr;
+    }
+    ~OptScratch()
+    {
+        if (big) {   // the unit must leave its table zero for the next holder of the slot
+            const lzb::u32* t = (const lzb::u32*)big;
+            for (size_t i = 0; i < lzb::kLpBigTableBytes / 4; ++i) LZB_SHIM_CHECK(t[i] == 0);
+        }
+        free(work->lp.huf.seg_count); free(work); free(stats); free(big);
+    }
+};
+
 extern "C" int lzb_host_compress(const unsigned char* src, int n, unsigned char* dst, int cap, int level)
 {
     if (n < 0 || cap < 0) return 0;
@@ -79,6 +112,10 @@ extern "C" int lzb_host_compress(const unsigned char* src, int n, unsigned char*
     if (lzb::lp_level(level)) {
         LpScratch sc(n);
         return lzb::encode_unit_lp<lzb::HostLanes>(src, (lzb::u32)n, dst, (lzb::u32)cap, level, sc.work, 1, sc.big);
+    }
+    if (lzb::opt_level(level)) {
+        OptScratch sc(n);
+        return lzb::encode_unit_opt<lzb::HostLanes>(src, (lzb::u32)n, dst, (lzb::u32)cap, level, sc.work, 1, sc.big, sc.stats);
     }
     lzb::LevelParams lp = lzb::level_params(level);
     if (lp.parser == lzb::kParserUnsupported) return 0;
@@ -363,6 +400,15 @@ static void emu_lp_body(void* p)
     if (EmuLanes::lane() == 0) a->result = r;
 }
 
+struct EmuOptArgs { const unsigned char* src; int n; unsigned char* dst; int cap; int level; lzb::OptWork* work; lzb::u8* big;
+                    lzb::OptStats* stats; unsigned epoch; int result; };
+static void emu_opt_body(void* p)
+{
+    EmuOptArgs* a = (EmuOptArgs*)p;
+    int r = lzb::encode_unit_opt<EmuLanes>(a->src, (lzb::u32)a->n, a->dst, (lzb::u32)a->cap, a->level, a->work, a->epoch, a->big, a->stats);
+    if (EmuLanes::lane() == 0) a->result = r;
+}
+
 // Lizard_compress through the 32-lane emulation of the device code path
 extern "C" int lzb_emu_compress(const unsigned char* src, int n, unsigned char* dst, int cap, int level)
 {
@@ -373,6 +419,12 @@ extern "C" int lzb_emu_compress(const unsigned char* src, int n, unsigned char* 
         LpScratch sc(n);
         EmuLpArgs a = { src, n, dst, cap, level, &sc, 0 };
         emu::run(emu_lp_body, &a);
+        return a.result;
+    }
+    if (lzb::opt_level(level)) {
+        OptScratch sc(n);
+        EmuOptArgs a = { src, n, dst, cap, level, sc.work, sc.big, sc.stats, 1, 0 };
+        emu::run(emu_opt_body, &a);
         return a.result;
     }
     lzb::LevelParams lp = lzb::level_params(level);
@@ -425,11 +477,9 @@ extern "C" void lzb_lp_scratch_free(void* p)
 //    position p that the unit inserts, bucket(p) -> p - k (k = 1..7).  Taken for a current entry, such an entry lies within
 //    8 bytes below p, so Lizard_Insert's "replace unless within 8" rule keeps it instead of p, and the parse loses matches.
 // A map that counts every slot of another epoch as empty gives the unit the reference's bytes.
-extern "C" void lzb_lp_scratch_poison_map(void* p, unsigned epoch, unsigned hash_log, unsigned seed,
-                                          const unsigned char* src, int n, unsigned mls)
+static void poison_map(lzb::u64* const map, unsigned epoch, unsigned hash_log, unsigned seed, const unsigned char* src, int n,
+                       unsigned mls)
 {
-    LpPersist* sc = (LpPersist*)p;
-    lzb::u64* const map = sc->work->map;
     const lzb::u32 shift = hash_log - lzb::kLpMapLog, mx = lzb::kLpEpochMax, mask = (1u << lzb::kLpMapLog) - 1;
     lzb::u32 other[4] = { 0u, (epoch - 1) & mx, (epoch + 1) & mx, mx };
     for (lzb::u32& e : other)
@@ -452,6 +502,11 @@ extern "C" void lzb_lp_scratch_poison_map(void* p, unsigned epoch, unsigned hash
         map[i] = (lzb::u64)other[q & 3] << 41 | (lzb::u64)h << 18 | (stale + 1);
         placed[i] = 1;
     }
+}
+extern "C" void lzb_lp_scratch_poison_map(void* p, unsigned epoch, unsigned hash_log, unsigned seed,
+                                          const unsigned char* src, int n, unsigned mls)
+{
+    poison_map(((LpPersist*)p)->work->map, epoch, hash_log, seed, src, n, mls);
 }
 // the kernel's rule when a warp's epoch reaches kLpEpochMax: clear the map, go on at epoch 1
 extern "C" void lzb_lp_scratch_clear_map(void* p) { memset(((LpPersist*)p)->work->map, 0, sizeof ((LpPersist*)p)->work->map); }
@@ -479,6 +534,63 @@ extern "C" int lzb_lp_compress_on(void* p, const unsigned char* src, int n, unsi
     if (!emu) return lzb::encode_unit_lp<lzb::HostLanes>(src, (lzb::u32)n, dst, (lzb::u32)cap, level, sc->work, epoch, sc->big);
     EmuLpOnArgs a = { src, n, dst, cap, level, sc, epoch, 0 };
     emu::run(emu_lp_on_body, &a);
+    return a.result;
+}
+
+// ---- the optimal parser on persistent, poisoned scratch -------------------------------------------------------------
+// As above for levels 18, 19 and 39: the warp's tree, opt[], match list, sequence list, streams and token statistics keep
+// garbage (or the previous unit's contents), its map entries of other epochs, its big slot a zero table.
+struct OptPersist { lzb::OptWork* work; lzb::u8* big; lzb::u32 (*seg)[256]; lzb::OptStats* stats; };
+extern "C" void* lzb_opt_scratch_new(unsigned seed)
+{
+    OptPersist* sc = (OptPersist*)malloc(sizeof(OptPersist));
+    sc->work = (lzb::OptWork*)malloc(sizeof(lzb::OptWork));
+    sc->seg = (lzb::u32 (*)[256])malloc(4 * 256 * sizeof(lzb::u32));
+    sc->stats = (lzb::OptStats*)malloc(sizeof(lzb::OptStats));
+    lp_fill(sc->work, sizeof(lzb::OptWork), seed);
+    lp_fill(sc->seg, 4 * 256 * sizeof(lzb::u32), seed + 1);
+    lp_fill(sc->stats, sizeof(lzb::OptStats), seed + 2);
+    sc->work->lp.huf.seg_count = sc->seg;
+    memset(sc->work->lp.map, 0, sizeof sc->work->lp.map);
+    sc->big = (lzb::u8*)calloc(1, lzb::kLpBigSlotBytes);
+    lp_fill(sc->big + lzb::kLpBigTableBytes, lzb::kLpBigChainBytes, seed + 3);
+    return sc;
+}
+extern "C" void lzb_opt_scratch_free(void* p)
+{
+    OptPersist* sc = (OptPersist*)p;
+    free(sc->seg); free(sc->work); free(sc->stats); free(sc->big); free(sc);
+}
+// garbage again in the tree (every 16th node a (U32)-1 link), opt[] and the match list, as another launch may leave them
+extern "C" void lzb_opt_scratch_poison(void* p, unsigned seed)
+{
+    OptPersist* sc = (OptPersist*)p;
+    lp_fill(sc->work->lp.chain, sizeof sc->work->lp.chain, seed);
+    for (size_t i = 0; i < sizeof sc->work->lp.chain / 4; i += 16) sc->work->lp.chain[i] = lzb::kOptNoLink;
+    lp_fill(sc->work->opt, sizeof sc->work->opt, seed + 1);
+    lp_fill(sc->work->match, sizeof sc->work->match, seed + 2);
+}
+// the map poisoned as lzb_lp_scratch_poison_map does it (hash4 buckets)
+extern "C" void lzb_opt_scratch_poison_map(void* p, unsigned epoch, unsigned hash_log, unsigned seed, const unsigned char* src, int n)
+{
+    poison_map(((OptPersist*)p)->work->lp.map, epoch, hash_log, seed, src, n, 4);
+}
+extern "C" void lzb_opt_scratch_clear_map(void* p) { memset(((OptPersist*)p)->work->lp.map, 0, sizeof ((OptPersist*)p)->work->lp.map); }
+extern "C" int lzb_opt_scratch_big_clean(void* p)
+{
+    const lzb::u32* t = (const lzb::u32*)((OptPersist*)p)->big;
+    for (size_t i = 0; i < lzb::kLpBigTableBytes / 4; ++i) if (t[i]) return 0;
+    return 1;
+}
+// one unit at level 18, 19 or 39 on the persistent scratch under `epoch` (1 .. kLpEpochMax); emu = 32 emulated lanes
+extern "C" int lzb_opt_compress_on(void* p, const unsigned char* src, int n, unsigned char* dst, int cap, int level,
+                                   unsigned epoch, int emu)
+{
+    OptPersist* sc = (OptPersist*)p;
+    if (n < 0 || cap < 0 || !lzb::opt_level(level) || epoch < 1 || epoch > lzb::kLpEpochMax) return 0;
+    if (!emu) return lzb::encode_unit_opt<lzb::HostLanes>(src, (lzb::u32)n, dst, (lzb::u32)cap, level, sc->work, epoch, sc->big, sc->stats);
+    EmuOptArgs a = { src, n, dst, cap, level, sc->work, sc->big, sc->stats, epoch, 0 };
+    emu::run(emu_opt_body, &a);
     return a.result;
 }
 
