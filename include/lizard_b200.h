@@ -103,8 +103,13 @@ int Lizard_decompress_safe_usingDict(const char* source, char* dest, int compres
  *      lib/lizard_compress.h:178-198, lib/lizard_decompress.h:89-145) the DECODE side is implemented on the GPU:
  *      Lizard_setStreamDecode and Lizard_decompress_safe_continue keep the reference's window state (an external
  *      dictionary plus the prefix decoded in place, lib/lizard_decompress.c:303-344) and decode one unit per call against
- *      it, like Lizard_decompress_safe_usingDict (1).  The COMPRESS side is out of scope and fails with the reference's
- *      failure value: 0 from Lizard_loadDict / Lizard_saveDict / Lizard_compress_continue.  No CPU code path behind any.
+ *      it, like Lizard_decompress_safe_usingDict (1).  On the COMPRESS side, Lizard_loadDict records the dictionary in the
+ *      stream object and returns the reference's value (the size, trimmed to the last 2^24 bytes); the stream's next
+ *      Lizard_compress_continue is Lizard_loadDict + Lizard_compress_continue of the reference, byte for byte, in one launch
+ *      (LizardB200_compress_dict_batch; levels 13-17, 21, 22, 34-38, 41 and 42, other levels return 0).  Lizard_compress_continue on
+ *      a fresh or reset stream is Lizard_compress, at every GPU level.  Any later Lizard_compress_continue on the same stream
+ *      would need the tables the previous call left behind: it returns 0, as Lizard_saveDict always does.  No CPU code path
+ *      behind any.
  * ------------------------------------------------------------------------------------------- */
 typedef struct Lizard_stream_s Lizard_stream_t;                 /* lib/lizard_compress.h:72 */
 typedef struct Lizard_streamDecode_s Lizard_streamDecode_t;     /* lib/lizard_decompress.h:100 */
@@ -206,6 +211,19 @@ int LizardB200_decompress_partial_batch(const void* const* src, const int* compr
 int LizardB200_decompress_dict_batch(const void* const* src, const int* compressedSize,
                                      void* const* dst, const int* dstCapacity,
                                      const void* const* dict, const int* dictSize, int* result, int nUnits);
+/* result[i] as Lizard_createStream(level) + Lizard_loadDict(dict[i], dictSize[i]) + Lizard_compress_continue(src[i], dst[i],
+ * srcSize[i], dstCapacity[i]) of the reference, byte for byte; dictSize[i] == 0 means no dictionary (then as Lizard_compress).
+ * The dictionary is a prefix when dict[i] + dictSize[i] == src[i], as in the reference; an input that overlaps its dictionary
+ * limits the window as the reference does.  Units whose dictionaries end at the same address with the same size share one
+ * staged and loaded copy.  Levels 13-17 and 34-38 (hashChain), 21, 22, 41 and 42 (priceFast); LIZARDB200_ERR_LEVEL at every
+ * other level.
+ * LIZARDB200_ERR_MEMORY when the call has more distinct dictionaries of 8 bytes or more than the encode workspace holds slots
+ * for (each takes 1.125 MiB: 1883 for 5000 units on an 80 GB H100; LizardB200_lastError says how many).  One kernel launch
+ * (lizard_encode_dict_kernel: the first unit of each dictionary loads its table, the others wait for it), behind a memset of
+ * the dictionary map. */
+int LizardB200_compress_dict_batch(const void* const* src, const int* srcSize,
+                                   void* const* dst, const int* dstCapacity,
+                                   const void* const* dict, const int* dictSize, int* result, int nUnits, int compressionLevel);
 
 /* Contiguous host buffers, units described by offset/size arrays (what a frame or a file splitter has).
  * dstStride: unit i is written at dst + i*dstStride with capacity dstCapacityEach. */
@@ -240,6 +258,16 @@ int LizardB200_decompress_dict_device(const void* dSrc, const uint64_t* dSrcOff,
 int LizardB200_compress_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
                                void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
                                int* dResult, unsigned nUnits, int compressionLevel, void* cudaStream);
+/* LizardB200_compress_dict_batch on device arrays: unit i's dictionary is dDictLen[i] bytes at dDict + dDictOff[i] (0 = none);
+ * it is a prefix when dDict + dDictOff[i] + dDictLen[i] == dSrc + dSrcOff[i].  Enqueue-only, with the workspace and stream
+ * rules of LizardB200_compress_device.  A unit whose dictionary finds no slot in the workspace (more distinct dictionaries
+ * than the bound above) is not compressed and gets dResult[i] = -1; slots go to dictionaries in the order warps meet them, so
+ * which units those are depends on scheduling and may change from call to call.  Like the input, a dictionary may be read up to 8 bytes
+ * past its end. */
+int LizardB200_compress_dict_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
+                                    void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
+                                    const void* dDict, const uint64_t* dDictOff, const uint32_t* dDictLen,
+                                    int* dResult, unsigned nUnits, int compressionLevel, void* cudaStream);
 /* Concatenation step of a block writer on the device (what lib/lizard_frame.c:544-549 does by advancing dstPtr block by
  * block): segment i = dSrc + dSrcOff[i], dLen[i] bytes (entries <= 0 are skipped, e.g. failed units) is copied to
  * dDst + dDstOff[i].  With dLen = the result array of LizardB200_compress_device and dDstOff = its exclusive prefix sum this

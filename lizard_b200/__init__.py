@@ -56,6 +56,14 @@ def lib():
         L.LizardB200_decompress_partial_device.argtypes = [ctypes.c_void_p] * 8 + [ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_decompress_dict_device.argtypes = [ctypes.c_void_p] * 10 + [ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_compress_device.argtypes = dev_args + [ctypes.c_int, ctypes.c_void_p]
+        L.LizardB200_compress_dict_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int, ctypes.c_int]
+        L.LizardB200_compress_dict_device.argtypes = [ctypes.c_void_p] * 10 + [ctypes.c_uint, ctypes.c_int, ctypes.c_void_p]
+        L.Lizard_createStream.restype = ctypes.c_void_p
+        L.Lizard_createStream.argtypes = [ctypes.c_int]
+        L.Lizard_freeStream.argtypes = [ctypes.c_void_p]
+        L.Lizard_loadDict.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
+        L.Lizard_compress_continue.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int]
+        L.Lizard_saveDict.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
         L.LizardB200_gather_device.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_compress_blocks.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
@@ -150,6 +158,54 @@ def compress_batch(units, level, caps=None):
     return _batch(L.LizardB200_compress_batch, units, caps, (level,))
 
 
+def _dict_args(dicts, n):
+    """Per-unit dictionary pointers and sizes; units given the same bytes object share one buffer."""
+    if len(dicts) != n:
+        raise ValueError("one dictionary per unit")
+    ptrs, sizes, held = (ctypes.c_void_p * n)(), (ctypes.c_int * n)(), {}
+    for i, d in enumerate(dicts):
+        if d:
+            if id(d) not in held:
+                held[id(d)] = ctypes.create_string_buffer(bytes(d), len(d))
+            ptrs[i] = ctypes.addressof(held[id(d)])
+            sizes[i] = len(d)
+    return ptrs, sizes, held
+
+
+def compress_dict_batch(units, dicts, level, caps=None):
+    """LizardB200_compress_dict_batch: list of bytes, per-unit dictionary (bytes; b"" or None for none) -> list of (result,
+    compressed bytes), each as Lizard_loadDict + Lizard_compress_continue with an external dictionary.  Units given the same
+    bytes object share one dictionary buffer.  Levels 13-17, 21, 22, 34-38, 41 and 42."""
+    L = lib()
+    caps = [L.Lizard_compressBound(len(u)) for u in units] if caps is None else caps
+    ptrs, sizes, held = _dict_args(dicts, len(units))
+    return _batch(L.LizardB200_compress_dict_batch, units, caps, (level,), dicts=(ptrs, sizes))
+
+
+def compress_using_dict(src: bytes, dict: bytes, level: int, cap: int = None, prefix: bool = False) -> bytes:
+    """Lizard_createStream + Lizard_loadDict + Lizard_compress_continue on host bytes.  prefix=True lays the dictionary directly
+    in front of the input; otherwise it is an external dictionary.  Returns b'' when the library returns 0."""
+    L = lib()
+    cap = L.Lizard_compressBound(len(src)) if cap is None else cap
+    if prefix:
+        buf = ctypes.create_string_buffer(bytes(dict) + bytes(src), len(dict) + len(src) + 1)
+        dict_p, src_p = ctypes.addressof(buf), ctypes.addressof(buf) + len(dict)
+    else:
+        d = ctypes.create_string_buffer(bytes(dict), max(len(dict), 1))
+        s = ctypes.create_string_buffer(bytes(src), max(len(src), 1))
+        dict_p, src_p = ctypes.addressof(d), ctypes.addressof(s)
+    dst = ctypes.create_string_buffer(max(cap, 1))
+    st = L.Lizard_createStream(level)
+    if not st:
+        raise LizardB200Error("Lizard_createStream failed")
+    try:
+        L.Lizard_loadDict(st, dict_p, len(dict))
+        n = L.Lizard_compress_continue(st, src_p, dst, len(src), cap)
+    finally:
+        L.Lizard_freeStream(st)
+    return dst.raw[:n] if n > 0 else b""
+
+
 def decompress_batch(units, caps):
     """LizardB200_decompress_batch: list of compressed bytes -> list of (result, bytes)."""
     return _batch(lib().LizardB200_decompress_batch, units, caps, ())
@@ -167,16 +223,7 @@ def decompress_dict_batch(units, dicts, caps):
     """LizardB200_decompress_dict_batch: list of compressed bytes, per-unit dictionary (bytes; b"" or None for none) and
     capacity -> list of (result, bytes), each as decompress_using_dict with an external dictionary.  Units given the same
     bytes object share one dictionary buffer."""
-    if len(dicts) != len(units):
-        raise ValueError("one dictionary per unit")
-    n = len(units)
-    ptrs, sizes, held = (ctypes.c_void_p * n)(), (ctypes.c_int * n)(), {}
-    for i, d in enumerate(dicts):
-        if d:
-            if id(d) not in held:
-                held[id(d)] = ctypes.create_string_buffer(bytes(d), len(d))
-            ptrs[i] = ctypes.addressof(held[id(d)])
-            sizes[i] = len(d)
+    ptrs, sizes, held = _dict_args(dicts, len(units))
     return _batch(lib().LizardB200_decompress_dict_batch, units, caps, (), dicts=(ptrs, sizes))
 
 

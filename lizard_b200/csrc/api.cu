@@ -7,6 +7,7 @@
 #include "encode.cuh"
 #include "encode_lp_kernel.cuh"
 #include "encode_opt_kernel.cuh"
+#include "encode_dict_kernel.cuh"
 
 #include <cuda_runtime.h>
 #include <mutex>
@@ -14,6 +15,7 @@
 #include <functional>
 #include <vector>
 #include <unordered_map>
+#include <map>
 #include <utility>
 #include <string>
 #include <atomic>
@@ -577,6 +579,146 @@ int launch_encode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* d
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// levels with a dictionary path: the parsers that search a loaded dictionary through the table Lizard_loadDict fills
+// (dict_parser(), encode_core.cuh; kernel: encode_dict_kernel.cuh)
+bool enc_dict_level_ok(int level) { return dict_parser(level_params(level)); }
+const char* const kNoDictLevel = "compression with a dictionary is implemented on the GPU at levels 13-17, 21-22, 34-38 and 41-42 only "
+                                 "(the hashChain and priceFast parsers)";
+
+int launch_encode_dict(Context& c, const void* dSrc, const u64* dSrcOff, const u32* dSrcLen,
+                       void* dDst, const u64* dDstOff, const u32* dDstCap, const void* dDict, const u64* dDictOff,
+                       const u32* dDictLen, int* dResult, u32 n, int level, cudaStream_t s)
+{
+    if (!enc_dict_level_ok(level)) { g_last_error = kNoDictLevel; return LIZARDB200_ERR_LEVEL; }
+    if (n == 0) return LIZARDB200_OK;
+    if (dict_shape(c.enc_cfg, n).max_slots < 1) {
+        g_last_error = "the encode workspace has no room for a dictionary slot beside the warps' scratch";
+        return LIZARDB200_ERR_MEMORY;
+    }
+    workspace_acquire(c, s);
+    struct Release { Context& c; cudaStream_t s; ~Release() { workspace_release(c, s); } } release_on_exit{c, s};
+    EncodeBatch b;
+    memset(&b, 0, sizeof b);
+    b.src_base = (const u8*)dSrc; b.src_off = dSrcOff; b.src_len = dSrcLen;
+    b.dst_base = (u8*)dDst; b.dst_off = dDstOff; b.dst_cap = dDstCap;
+    b.result = dResult; b.n_units = n; b.level = level;
+    b.scratch = (u8*)c.enc_scratch.p;
+    b.counter = next_counter(c, s);
+    int launches = 0;
+    const cudaError_t e = dict_encode_launch(c.enc_cfg, b, (const u8*)dDict, dDictOff, dDictLen, s, &launches);
+    g_launches += (unsigned long long)launches;
+    if (e != cudaSuccess) { fail("dictionary encode launch", e); return LIZARDB200_ERR_CUDA; }
+    return LIZARDB200_OK;
+}
+
+// LizardB200_compress_dict_batch: every unit and its dictionary staged so that their relative placement survives: a unit that
+// touches or overlaps its dictionary (the prefix layout, or an input inside its dictionary) is staged together with it as one
+// range; other dictionaries are staged once per (end address, size).  Only the last 2^24 bytes of a dictionary are staged.
+int run_host_compress_dict(const void* const* src, const int* srcSize, void* const* dst, const int* dstCap,
+                           const void* const* dict, const int* dictSize, int* result, int n, int level)
+{
+    if (n < 0 || (n > 0 && (!src || !srcSize || !dst || !dstCap || !result || !dict || !dictSize))) return LIZARDB200_ERR_ARGUMENT;
+    Context& c = g_ctx[g_device];
+    std::lock_guard<std::mutex> lock(c.mu);
+    int st = ensure_context(c, g_device);
+    if (st != LIZARDB200_OK) return st;
+    if (!enc_dict_level_ok(level)) { g_last_error = kNoDictLevel; return LIZARDB200_ERR_LEVEL; }
+    if (n == 0) return LIZARDB200_OK;
+    struct Range { const u8* lo; size_t bytes; u64 at; };
+    std::vector<Range> ranges;
+    std::map<std::pair<const u8*, u32>, size_t> shared;              // (end, size) -> range of a dictionary staged alone
+    std::vector<size_t> unit_range(n), dict_range(n);
+    std::vector<u32> dlen(n);
+    std::vector<const u8*> dptr(n);
+    size_t distinct = 0, out_total = 0;                               // dictionaries of 8 bytes or more; smaller ones share a slot
+    bool small = false;
+    std::vector<u64> out_off(n);
+    for (int i = 0; i < n; ++i) {
+        if (srcSize[i] < 0 || dstCap[i] < 0 || dictSize[i] < 0 || (srcSize[i] && !src[i]) || (dictSize[i] && !dict[i]))
+            return LIZARDB200_ERR_ARGUMENT;
+        const u8* s0 = (const u8*)src[i];
+        const u8* d0 = (const u8*)dict[i];
+        u32 dl = (u32)dictSize[i];
+        if (dl > kDictSize) { d0 += dl - kDictSize; dl = kDictSize; }
+        dptr[i] = d0; dlen[i] = dl;
+        out_off[i] = out_total; out_total += align_up((size_t)dstCap[i] + 32, 16);
+        small = small || dl < 8;
+        if (dl && s0 <= d0 + dl && s0 + srcSize[i] >= d0) {
+            const u8* lo = s0 < d0 ? s0 : d0;
+            const u8* hi = s0 + srcSize[i] > d0 + dl ? s0 + srcSize[i] : d0 + dl;
+            unit_range[i] = dict_range[i] = ranges.size();
+            ranges.push_back(Range{lo, (size_t)(hi - lo), 0});
+            distinct += dl >= 8;
+            continue;
+        }
+        unit_range[i] = ranges.size();
+        ranges.push_back(Range{s0, (size_t)srcSize[i], 0});
+        if (!dl) continue;
+        auto it = shared.find({d0 + dl, dl});
+        if (it == shared.end()) {
+            it = shared.emplace(std::make_pair(d0 + dl, dl), ranges.size()).first;
+            ranges.push_back(Range{d0, dl, 0});
+            distinct += dl >= 8;
+        }
+        dict_range[i] = it->second;
+    }
+    const DictShape shape = dict_shape(c.enc_cfg, (u32)n);
+    if (distinct + (small ? 1 : 0) > shape.max_slots) {
+        char buf[200];
+        snprintf(buf, sizeof buf, "%zu distinct dictionaries of 8 bytes or more in one call; the encode workspace holds %u for %d units",
+                 distinct, shape.max_slots - (small ? 1 : 0), n);
+        g_last_error = buf;
+        return LIZARDB200_ERR_MEMORY;
+    }
+    size_t in_total = 0;
+    for (Range& r : ranges) { r.at = in_total; in_total = align_up(in_total + r.bytes + 16, 16); }
+    const size_t tab_bytes = (size_t)n * (8 + 8 + 8 + 4 + 4 + 4 + 4);
+    CU_OK(c.pin_in.reserve(in_total));
+    CU_OK(c.pin_tab.reserve(tab_bytes));
+    CU_OK(c.d_in.reserve(in_total));
+    CU_OK(c.d_out.reserve(out_total));
+    CU_OK(c.d_tab.reserve(tab_bytes));
+    CU_OK(c.pin_out.reserve(out_total));
+    u64* t_in_off = (u64*)c.pin_tab.p;
+    u64* t_out_off = t_in_off + n;
+    u64* t_dict_off = t_out_off + n;
+    u32* t_in_len = (u32*)(t_dict_off + n);
+    u32* t_out_cap = t_in_len + n;
+    u32* t_dict_len = t_out_cap + n;
+    int* t_res = (int*)(t_dict_len + n);
+    for (const Range& r : ranges) if (r.bytes) memcpy((u8*)c.pin_in.p + r.at, r.lo, r.bytes);
+    for (int i = 0; i < n; ++i) {
+        const Range& ur = ranges[unit_range[i]];
+        t_in_off[i] = ur.at + (u64)((const u8*)src[i] - ur.lo);
+        t_out_off[i] = out_off[i];
+        t_in_len[i] = (u32)srcSize[i]; t_out_cap[i] = (u32)dstCap[i];
+        t_dict_len[i] = dlen[i];
+        t_dict_off[i] = dlen[i] ? ranges[dict_range[i]].at + (u64)(dptr[i] - ranges[dict_range[i]].lo) : 0;
+    }
+    u8* dtab = (u8*)c.d_tab.p;
+    cudaStream_t s = c.stream;
+    CU_OK(cudaMemcpyAsync(c.d_in.p, c.pin_in.p, in_total, cudaMemcpyHostToDevice, s));
+    CU_OK(cudaMemcpyAsync(dtab, c.pin_tab.p, tab_bytes - (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    const u64* d_in_off = (const u64*)dtab;
+    const u64* d_out_off = d_in_off + n;
+    const u64* d_dict_off = d_out_off + n;
+    const u32* d_in_len = (const u32*)(d_dict_off + n);
+    const u32* d_out_cap = d_in_len + n;
+    const u32* d_dict_len = d_out_cap + n;
+    int* d_res = (int*)(d_dict_len + n);
+    st = launch_encode_dict(c, c.d_in.p, d_in_off, d_in_len, c.d_out.p, d_out_off, d_out_cap, c.d_in.p, d_dict_off, d_dict_len,
+                            d_res, (u32)n, level, s);
+    if (st != LIZARDB200_OK) return st;
+    CU_OK(cudaMemcpyAsync(t_res, d_res, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    CU_OK(cudaMemcpyAsync(c.pin_out.p, c.d_out.p, out_total, cudaMemcpyDeviceToHost, s));
+    CU_OK(cudaStreamSynchronize(s));
+    for (int i = 0; i < n; ++i) {
+        result[i] = t_res[i];
+        if (result[i] > 0) memcpy(dst[i], (u8*)c.pin_out.p + out_off[i], (size_t)t_res[i]);
+    }
+    return LIZARDB200_OK;
+}
+
 // Shared body of the host-pointer batch calls: stage inputs + tables, run, fetch results + outputs.
 // `target` (decode only): per-unit targetOutputSize of a partial decode, null for a full one.
 // `dict` / `dictSize` (decode only): per-unit dictionary of Lizard_decompress_safe_usingDict, null for none.  Only the bytes
@@ -814,6 +956,20 @@ int LizardB200_compress_device(const void* dSrc, const uint64_t* dSrcOff, const 
     return launch_encode(c, dSrc, (const u64*)dSrcOff, dSrcLen, dDst, (const u64*)dDstOff, dDstCap, dResult, nUnits, level, (cudaStream_t)stream);
 }
 
+int LizardB200_compress_dict_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
+                                    void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
+                                    const void* dDict, const uint64_t* dDictOff, const uint32_t* dDictLen,
+                                    int* dResult, unsigned nUnits, int level, void* stream)
+{
+    if (nUnits > 0 && (!dDictOff || !dDictLen)) return LIZARDB200_ERR_ARGUMENT;
+    Context& c = g_ctx[g_device];
+    std::lock_guard<std::mutex> lock(c.mu);
+    int st = ensure_context(c, g_device);
+    if (st != LIZARDB200_OK) return st;
+    return launch_encode_dict(c, dSrc, (const u64*)dSrcOff, dSrcLen, dDst, (const u64*)dDstOff, dDstCap, dDict, (const u64*)dDictOff,
+                              dDictLen, dResult, nUnits, level, (cudaStream_t)stream);
+}
+
 int LizardB200_gather_device(const void* dSrc, const uint64_t* dSrcOff, const int* dLen,
                              void* dDst, const uint64_t* dDstOff, unsigned nUnits, void* stream)
 {
@@ -852,6 +1008,12 @@ int LizardB200_compress_batch(const void* const* src, const int* srcSize, void* 
                               int* result, int n, int level)
 {
     return run_host_batch<true>(src, srcSize, dst, dstCap, result, n, level);
+}
+
+int LizardB200_compress_dict_batch(const void* const* src, const int* srcSize, void* const* dst, const int* dstCap,
+                                   const void* const* dict, const int* dictSize, int* result, int n, int level)
+{
+    return run_host_compress_dict(src, srcSize, dst, dstCap, dict, dictSize, result, n, level);
 }
 
 
@@ -967,24 +1129,30 @@ int Lizard_compress_extState(void* state, const char* src, char* dst, int srcSiz
 
 // ---- the rest of lib/dll/liblizard.def: what callers of the block API link against -------------------------------------
 // Stream OBJECTS are functional (the reference's frame layer creates one per context and hands it to
-// Lizard_compress_extState, lib/lizard_frame.c:379-401, 436-451); the device keeps the real state, so the object only
-// records its level.  Dictionary and streamed DECODING run on the GPU (Lizard_decompress_safe_usingDict, _continue); the
-// compress side of the family (Lizard_loadDict, Lizard_saveDict, Lizard_compress_continue) is out of scope (SURVEY.md
-// section 2): those entry points exist so that the reference's own callers link, and they fail with the reference's failure
-// value 0, never with a CPU code path.
-struct Lizard_stream_s { size_t allocatedMemory; int compressionLevel; };
+// Lizard_compress_extState, lib/lizard_frame.c:379-401, 436-451); the device keeps the real state, so the object records the
+// level and what Lizard_loadDict was given.  Dictionary and streamed DECODING run on the GPU (Lizard_decompress_safe_usingDict,
+// _continue).  On the compress side, a stream's FIRST Lizard_compress_continue runs on the GPU: after Lizard_loadDict it is the
+// dictionary path (hashChain and priceFast levels), on a fresh or reset stream it is Lizard_compress (lib/lizard_compress.c:557).  Any later
+// _continue would need the tables the previous call left behind, and Lizard_saveDict moves them: both fail with the reference's
+// failure value 0, never with a CPU code path.
+struct Lizard_stream_s {
+    size_t allocatedMemory; int compressionLevel;
+    int state;                        // kStreamFresh, kStreamDict (Lizard_loadDict ran) or kStreamSpent
+    const char* dict; int dictSize;   // as given to Lizard_loadDict
+};
+enum { kStreamFresh = 0, kStreamDict = 1, kStreamSpent = 2 };
 struct Lizard_streamDecode_s {                                   // lib/lizard_common.h:195-200
     const u8* externalDict; size_t extDictSize;
     const u8* prefixEnd; size_t prefixSize;
 };
-static const char* const kNoStreaming = "streaming compression with a dictionary (linked blocks) is not implemented on the GPU path";
+static const char* const kNoStreaming = "streaming compression across calls (linked blocks, Lizard_saveDict) is not implemented on the GPU path";
 
 Lizard_stream_t* Lizard_createStream(int level)            // lib/lizard_compress.c:392-397
 {
     if (level > (int)kMaxLevel) level = kMaxLevel;
     if (level < (int)kMinLevel) level = kDefaultLevel;
     Lizard_stream_t* p = (Lizard_stream_t*)malloc(sizeof(Lizard_stream_t));
-    if (p) { p->allocatedMemory = sizeof(Lizard_stream_t); p->compressionLevel = level; }
+    if (p) { p->allocatedMemory = sizeof(Lizard_stream_t); p->compressionLevel = level; p->state = kStreamFresh; p->dict = nullptr; p->dictSize = 0; }
     return p;
 }
 int Lizard_freeStream(Lizard_stream_t* p) { free(p); return 0; }              // :417-423
@@ -994,11 +1162,28 @@ Lizard_stream_t* Lizard_resetStream(Lizard_stream_t* p, int level)            //
     if (level > (int)kMaxLevel) level = kMaxLevel;
     if (level < (int)kMinLevel) level = kDefaultLevel;
     p->compressionLevel = level;
+    p->state = kStreamFresh; p->dict = nullptr; p->dictSize = 0;
     return p;
 }
-int Lizard_loadDict(Lizard_stream_t*, const char*, int) { g_last_error = kNoStreaming; return 0; }
-int Lizard_saveDict(Lizard_stream_t*, char*, int) { g_last_error = kNoStreaming; return 0; }
-int Lizard_compress_continue(Lizard_stream_t*, const char*, char*, int, int) { g_last_error = kNoStreaming; return 0; }
+int Lizard_loadDict(Lizard_stream_t* p, const char* dictionary, int dictSize)   // :426-437
+{
+    if (dictSize > (int)kDictSize) { dictionary += dictSize - (int)kDictSize; dictSize = (int)kDictSize; }
+    p->state = dictSize >= 0 ? kStreamDict : kStreamSpent;
+    p->dict = dictionary; p->dictSize = dictSize;
+    return dictSize;
+}
+int Lizard_saveDict(Lizard_stream_t* p, char*, int) { p->state = kStreamSpent; g_last_error = kNoStreaming; return 0; }
+int Lizard_compress_continue(Lizard_stream_t* p, const char* src, char* dst, int srcSize, int maxDstSize)   // :550-580
+{
+    const int state = p->state;
+    p->state = kStreamSpent;
+    if (state == kStreamFresh) return Lizard_compress(src, dst, srcSize, maxDstSize, p->compressionLevel);
+    if (state != kStreamDict) { g_last_error = kNoStreaming; return 0; }
+    if (srcSize < 0 || maxDstSize < 0) return 0;
+    const void* s = src; void* d = dst; const void* dict = p->dict; int r = 0;
+    const int st = LizardB200_compress_dict_batch(&s, &srcSize, &d, &maxDstSize, &dict, &p->dictSize, &r, 1, p->compressionLevel);
+    return st == LIZARDB200_OK ? r : 0;
+}
 
 Lizard_streamDecode_t* Lizard_createStreamDecode(void) { return (Lizard_streamDecode_t*)calloc(1, sizeof(Lizard_streamDecode_t)); }
 int Lizard_freeStreamDecode(Lizard_streamDecode_t* p) { free(p); return 0; }

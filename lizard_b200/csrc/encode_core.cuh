@@ -266,6 +266,7 @@ struct HashTable {       // runtime descriptor handed to encode_unit
 };
 struct PlainTable {
     static constexpr bool kOneBlock = false;    // any unit
+    static constexpr bool kDict = false;        // positions start at the unit (DictTable: at a loaded dictionary)
     u32* t32; u32 tagged;
     LZ_HDM explicit PlainTable(const HashTable& d) : t32(d.t32), tagged(d.tagged) {}
     LZ_HDM u32 get(u32 h, u32) const { const u32 e = t32[h]; return tagged ? e & 0x1FFFFFFu : e; }
@@ -288,6 +289,7 @@ struct PlainTable {
 };
 struct PackedTable {
     static constexpr bool kOneBlock = true;     // units of one inner block only (positions below 2^17)
+    static constexpr bool kDict = false;
     u16* lo; u32* hi; u8* tag;
     LZ_HDM explicit PackedTable(const HashTable& d) : lo(d.lo), hi(d.hi), tag(d.tag) {}
     LZ_HDM u32 get(u32 h, u32 pos_hint) const
@@ -320,6 +322,36 @@ struct PackedTable {
         W::sync();                                  // tags of empty entries are never looked at
     }
 };
+// hashChain and priceFast against a loaded dictionary (Lizard_loadDict + Lizard_compress_continue, lib/lizard_compress.c:426-450,
+// 550-580).
+// Positions count from the dictionary's first byte: the dictionary is [0, dend), the unit starts at dend, and an entry is
+// position + kDictSize, the reference's own index.  The table after Lizard_loadDict is built once per dictionary and shared
+// read-only by every unit that uses it (`sh`, with the chain entries of the positions it inserted in `dchain`); a unit writes
+// only its own overlay `ov`, where 0 means "not written by this unit": every write a unit makes stores one of its own
+// positions (>= own0), so an empty overlay entry is exactly a bucket the unit has not changed.  The overlay is cleared per
+// unit as the plain table is.  ext: the dictionary is external (Lizard_setExternalDict ran) and its bytes are at dsrc;
+// otherwise it lies directly in front of the unit and dsrc is the parse's own base.
+struct DictTable {
+    static constexpr bool kOneBlock = false;
+    static constexpr bool kDict = true;
+    u32* ov; const u32* sh; const u16* dchain; const u8* dsrc;
+    u32 dend;            // dictionary size (= the unit's first position)
+    u32 own0;            // hashChain's nextToUpdate: dend, or dend - 7 for a prefix dictionary (priceFast writes positions >= dend)
+    u32 low;             // ctx->lowLimit as an index
+    u32 ext;
+    LZ_HDM u32 get(u32 h, u32) const { const u32 e = ov[h]; return e ? e : sh[h]; }
+    LZ_HDM void set(u32 h, u32 abs_index) const { if (abs_index >= own0 + kDictSize) ov[h] = abs_index; }
+    LZ_HDM u32 get_t(u32 h, u32 pos_hint, u32* t) const { *t = kNoTag; return get(h, pos_hint); }      // priceFast: no tags
+    LZ_HDM void set_t(u32 h, u32 abs_index, u32) const { set(h, abs_index); }
+    LZ_HDM bool maybe(u32, u32) const { return true; }
+    template <class W> LZ_HDM void clear(u32 hash_log) const
+    {
+        const u32 n = 1u << hash_log;
+        for (u32 i = W::lane(); i < n; i += W::lanes()) ov[i] = 0;
+        W::sync();
+    }
+};
+
 // Which tables carry tags: the plain table has the bits to spare (fast parsers and priceFast use them; single-block units
 // only); a packed table pays a byte per entry, which the small level-10/30 tables of the fast parsers are given and the
 // 34 KiB priceFast tables are not.
@@ -745,12 +777,56 @@ template <class W, class TT> LZ_HD void hc_insert(const u8* src, const TT& T, u3
     }
     cs.next_insert = upto;
 }
+// DictTable helpers.  Lizard_count_2segments (lizard_compress.c:118-124): a match read from the external dictionary that
+// reaches its end goes on at the unit's first byte.
+template <class W> LZ_HD u32 count_2seg(const u8* a, const u8* b, const u8* a_limit, const u8* b_end, const u8* a_start)
+{
+    const u8* v_end = (size_t)(b_end - b) < (size_t)(a_limit - a) ? a + (b_end - b) : a_limit;
+    const u32 n = count_match_par<W>(a, b, v_end);
+    if (b + n != b_end) return n;
+    return n + count_match_par<W>(a + n, a_start, a_limit);
+}
+template <class W> LZ_HD u32 count_2seg_1(const u8* a, const u8* b, const u8* a_limit, const u8* b_end, const u8* a_start)
+{   // the same with one lane
+    const u8* v_end = (size_t)(b_end - b) < (size_t)(a_limit - a) ? a + (b_end - b) : a_limit;
+    const u32 n = count_match(a, b, v_end);
+    if (b + n != b_end) return n;
+    return n + count_match(a + n, a_start, a_limit);
+}
+#if defined(LZB_DICT_ENC_STATS) && !defined(__CUDA_ARCH__)
+// host shim only: matches of the priceFast dictionary parse that start in the dictionary (tests prove both kinds occur)
+enum { kDictRepInDict, kDictMatchInDict, kDictEncStats };
+extern unsigned long long g_dict_enc_stats[kDictEncStats];
+#define LZB_DICT_COUNT(k) do { if (W::lane() == 0) g_dict_enc_stats[k]++; } while (0)
+#else
+#define LZB_DICT_COUNT(k) do { } while (0)
+#endif
+// backward extension with the two sides in different buffers: a[ip - k] against b[mpos - k], ip - k >= floor, mpos - k >= mlow
+template <class W> LZ_HD u32 extend_back_2seg(const u8* a, u32 ip, const u8* b, u32 mpos, u32 floor, u32 mlow)
+{
+    u32 done = 0;
+    for (;;) {
+        const u32 k = done + W::lane() + 1;
+        const bool can = ip >= floor + k && mpos >= mlow + k;
+        const bool eq = can && a[ip - k] == b[mpos - k];
+        const u32 bad = W::ballot(!eq);
+        if (bad) return done + ctz32(bad);
+        done += W::lanes();
+    }
+}
+template <class TT> LZ_HD u32 hc_next(const TT& T, const ChainState& cs, u32 c)
+{
+    if constexpr (TT::kDict) { if (c < T.own0) return T.dchain[c & 0xFFFFu]; }   // inserted by Lizard_loadDict
+    return cs.chain[c & cs.chain_mask];
+}
+
 // Lizard_InsertAndFindBestMatch (:45-106); returns the length (0 = none), *ref = match position
 template <class W, class TT> LZ_HD u32 hc_best(const u8* src, const TT& T, u32 hl, u32 max_dist, ChainState& cs,
                                                u32 ip, const u8* limit, u32* ref)
 {
     const u32 bias = kDictSize, cur = ip + bias;
-    const u32 low = (bias + max_dist >= cur) ? bias : cur - max_dist;
+    u32 low = (bias + max_dist >= cur) ? bias : cur - max_dist;
+    if constexpr (TT::kDict) low = (T.low + max_dist >= cur) ? T.low : cur - max_dist;
     hc_insert<W, TT>(src, T, hl, max_dist, cs, ip);
     u32 m = T.get(hc_hash(src + ip, hl, cs.mls), ip);
     u32 tries = cs.search_num, best = 0;
@@ -758,11 +834,20 @@ template <class W, class TT> LZ_HD u32 hc_best(const u8* src, const TT& T, u32 h
     while (m < cur && m >= low && tries) {
         const u32 c = m - bias;
         tries--;
-        if (ip - c >= kMinOffset && src[c + best] == src[ip + best] && ld32(src + c) == v) {
+        bool ext_dict = false;
+        if constexpr (TT::kDict) ext_dict = T.ext && c < T.dend;
+        if (ext_dict) {                                  // the external dictionary's branch (:85-97)
+            if constexpr (TT::kDict) {
+                if (ip - c >= kMinOffset && T.dend - 1 - c >= 3 && ld32(T.dsrc + c) == v) {
+                    const u32 len = count_2seg<W>(src + ip + kMinMatch, T.dsrc + c + kMinMatch, limit, T.dsrc + T.dend, src + T.dend) + kMinMatch;
+                    if (len > best) { best = len; *ref = c; }
+                }
+            }
+        } else if (ip - c >= kMinOffset && src[c + best] == src[ip + best] && ld32(src + c) == v) {
             const u32 len = count_match_par<W>(src + ip + kMinMatch, src + c + kMinMatch, limit) + kMinMatch;
             if (len > best) { best = len; *ref = c; }
         }
-        const u32 d = cs.chain[c & cs.chain_mask];
+        const u32 d = hc_next(T, cs, c);
         if (d > m) break;
         m -= d;
     }
@@ -773,7 +858,8 @@ template <class W, class TT> LZ_HD u32 hc_wider(const u8* src, const TT& T, u32 
                                                 u32 ip, u32 floor, const u8* limit, u32 longest, u32* ref, u32* start)
 {
     const u32 bias = kDictSize, cur = ip + bias;
-    const u32 low = (bias + max_dist >= cur) ? bias : cur - max_dist;
+    u32 low = (bias + max_dist >= cur) ? bias : cur - max_dist;
+    if constexpr (TT::kDict) low = (T.low + max_dist >= cur) ? T.low : cur - max_dist;
     const u32 lead = ip - floor;
     hc_insert<W, TT>(src, T, hl, max_dist, cs, ip);
     u32 m = T.get(hc_hash(src + ip, hl, cs.mls), ip);
@@ -782,14 +868,29 @@ template <class W, class TT> LZ_HD u32 hc_wider(const u8* src, const TT& T, u32 
     while (m < cur && m >= low && tries) {
         const u32 c = m - bias;
         tries--;
+        bool ext_dict = false;
+        if constexpr (TT::kDict) ext_dict = T.ext && c < T.dend;
+        if (ext_dict) {                                  // the external dictionary's branch (:158-170): back down to the window
+            if constexpr (TT::kDict) {
+                if (ip - c >= kMinOffset && T.dend - 1 - c >= 3 && ld32(T.dsrc + c) == v) {
+                    u32 len = kMinMatch + count_2seg<W>(src + ip + kMinMatch, T.dsrc + c + kMinMatch, limit, T.dsrc + T.dend, src + T.dend);
+                    const u32 back = extend_back_2seg<W>(src, ip, T.dsrc, c, floor, low - bias);
+                    len += back;
+                    if (len > longest) { longest = len; *ref = c - back; *start = ip - back; }
+                }
+            }
         // c - lead + longest >= c + 3 in both call sites (lead = longest - 3), so the probe stays inside the unit
-        if (ip - c >= kMinOffset && src[floor + longest] == src[c - lead + longest] && ld32(src + c) == v) {
+        } else if (ip - c >= kMinOffset && src[floor + longest] == src[c - lead + longest] && ld32(src + c) == v) {
             u32 len = kMinMatch + count_match_par<W>(src + ip + kMinMatch, src + c + kMinMatch, limit);
-            const u32 back = extend_back_par<W>(src, ip, c, floor);
+            u32 back;
+            if constexpr (TT::kDict) {   // back down to lowPrefixPtr: the unit's start, or the prefix dictionary's
+                const u32 p0 = T.ext ? T.dend : 0u;
+                back = extend_back_par<W>(src + p0, ip - p0, c - p0, floor - p0);
+            } else back = extend_back_par<W>(src, ip, c, floor);
             len += back;
             if (len > longest) { longest = len; *ref = c - back; *start = ip - back; }
         }
-        const u32 d = cs.chain[c & cs.chain_mask];
+        const u32 d = hc_next(T, cs, c);
         if (d > m) break;
         m -= d;
     }
@@ -886,6 +987,15 @@ template <class W, class TT> LZ_HD_COLD void parse_hash_chain(const ParseCtx<TT>
     emit_last_literals<W>(st, src, anchor, b1);
 }
 
+// priceFast's backward extension against a loaded dictionary: down to lowPrefixPtr (:177, :195), the unit's start or the prefix
+// dictionary's.  A candidate in an external dictionary lies below lowPrefixPtr as a virtual pointer, so it never extends.
+template <class W> LZ_HD u32 dict_back(const DictTable& T, const u8* src, u32 ip, u32 ref, u32 floor)
+{
+    if (T.ext && ref < T.dend) return 0;
+    const u32 p0 = T.ext ? T.dend : 0u;
+    return extend_back_par<W>(src + p0, ip - p0, ref - p0, floor - p0);
+}
+
 // Lizard_compress_priceFast with the no-match run probed W::lanes() consecutive positions at a time.
 // Per position the reference (lizard_parser_pricefast.h:158-173) tests the repeat offset first, then the
 // bucket's candidate, then conditionally refreshes the bucket.  last_off is constant during a no-match run,
@@ -915,7 +1025,8 @@ template <class W, class TT> LZ_HD void parse_price_fast_par(const ParseCtx<TT>&
             const u32 P = ip + lane;
             const bool valid = P < mflimit;
             const u32 cur = P + bias;
-            const u32 low = (bias + max_dist >= cur) ? bias : cur - max_dist;
+            u32 low = (bias + max_dist >= cur) ? bias : cur - max_dist;
+            if constexpr (TT::kDict) low = (T.low + max_dist >= cur) ? T.low : cur - max_dist;
             u64 v = 0; u32 h = 0x80000000u | lane;
             if (valid) { v = (ahead_pos == P) ? v_ahead : ld5(src + P); h = hash5(v, hl); }
             {   // request the bytes of the following NL positions one batch early (used if this batch finds nothing)
@@ -938,18 +1049,31 @@ template <class W, class TT> LZ_HD void parse_price_fast_par(const ParseCtx<TT>&
             const u32 seen_v = W::shfl((u32)v, seen_lane < NL ? seen_lane : lane);
             bool rep_hit = false, hash_hit = false;
             if (valid) {
-                if (last_off >= kMinOffset && last_off <= P && cur - last_off >= low)
-                    rep_hit = ld32(src + (P - last_off)) == (u32)v;
+                if (last_off >= kMinOffset && last_off <= P && cur - last_off >= low) {
+                    bool ext_dict = false;
+                    if constexpr (TT::kDict) ext_dict = T.ext && P - last_off < T.dend;
+                    if (ext_dict) {                            // the external dictionary's branch (lizard_parser_pricefast.h:32-42)
+                        if constexpr (TT::kDict)
+                            rep_hit = T.dend - 1 - (P - last_off) >= 3 && ld32(T.dsrc + (P - last_off)) == (u32)v;
+                    } else rep_hit = ld32(src + (P - last_off)) == (u32)v;
+                }
                 if (!rep_hit && seen < cur && seen >= low) {
                     const u32 m = seen - bias;
-                    bool eq4 = false;
+                    bool eq4 = false, ext_dict = false;
+                    if constexpr (TT::kDict) ext_dict = T.ext && m < T.dend;
                     if (P - m >= kMinOffset) {
                         if (seen_lane < NL) eq4 = seen_v == (u32)v;
-                        else if (T.maybe(ttag, mytag)) eq4 = ld32(src + m) == (u32)v;
+                        else if (ext_dict) {                   // :76-85
+                            if constexpr (TT::kDict) eq4 = T.dend - 1 - m >= 3 && ld32(T.dsrc + m) == (u32)v;
+                        } else if (T.maybe(ttag, mytag)) eq4 = ld32(src + m) == (u32)v;
                     }
                     if (eq4) {
                         if (P - m < kMax16BitOffset) hash_hit = true;
-                        else hash_hit = count_match(src + P + kMinMatch, src + m + kMinMatch, matchlimit) + kMinMatch >= min_match_long;
+                        else if (ext_dict) {
+                            if constexpr (TT::kDict)
+                                hash_hit = count_2seg_1<W>(src + P + kMinMatch, T.dsrc + m + kMinMatch, matchlimit, T.dsrc + T.dend,
+                                                           src + T.dend) + kMinMatch >= min_match_long;
+                        } else hash_hit = count_match(src + P + kMinMatch, src + m + kMinMatch, matchlimit) + kMinMatch >= min_match_long;
                     }
                 }
             }
@@ -971,13 +1095,23 @@ template <class W, class TT> LZ_HD void parse_price_fast_par(const ParseCtx<TT>&
             ip = W::shfl(P, w_lane);
             const u32 is_rep = W::shfl(rep_hit ? 1u : 0u, w_lane);
             ref = is_rep ? ip - last_off : W::shfl(seen, w_lane) - bias;
-            ml = count_match_par<W>(src + ip + kMinMatch, src + ref + kMinMatch, matchlimit) + kMinMatch;
+            if constexpr (TT::kDict) {
+                if (ref < T.dend) LZB_DICT_COUNT(is_rep ? kDictRepInDict : kDictMatchInDict);
+                if (T.ext && ref < T.dend)
+                    ml = count_2seg<W>(src + ip + kMinMatch, T.dsrc + ref + kMinMatch, matchlimit, T.dsrc + T.dend, src + T.dend) + kMinMatch;
+                else ml = count_match_par<W>(src + ip + kMinMatch, src + ref + kMinMatch, matchlimit) + kMinMatch;
+            } else ml = count_match_par<W>(src + ip + kMinMatch, src + ref + kMinMatch, matchlimit) + kMinMatch;
         }
 
         u32 ml2 = 0, start2 = 0, ref2 = 0;
         bool encode_now = false;
         if (ip - ref == last_off) { ref = ip; encode_now = true; }
-        else { const u32 back = extend_back_par<W>(src, ip, ref, anchor); ip -= back; ref -= back; ml += back; }
+        else {
+            u32 back;
+            if constexpr (TT::kDict) back = dict_back<W>(T, src, ip, ref, anchor);
+            else back = extend_back_par<W>(src, ip, ref, anchor);
+            ip -= back; ref -= back; ml += back;
+        }
 
         for (;;) {
             if (!encode_now) {
@@ -986,27 +1120,40 @@ template <class W, class TT> LZ_HD void parse_price_fast_par(const ParseCtx<TT>&
                     start2 = ip + ml - 2;
                     {   // Lizard_FindMatchFaster (uniform: one position)
                         const u32 cur2 = start2 + bias;
-                        const u32 low2 = (bias + max_dist >= cur2) ? bias : cur2 - max_dist;
+                        u32 low2 = (bias + max_dist >= cur2) ? bias : cur2 - max_dist;
+                        if constexpr (TT::kDict) low2 = (T.low + max_dist >= cur2) ? T.low : cur2 - max_dist;
                         const u64 v2 = ld5(src + start2);
                         const u32 h2 = hash5(v2, hl);
                         u32 tag2 = kNoTag;
                         const u32 cand2 = T.get_t(h2, start2, &tag2);
                         ml2 = 0;
-                        bool ok = false; u32 m = 0;
+                        bool ok = false, ext_dict = false; u32 m = 0;
                         if (cand2 < cur2 && cand2 >= low2) {
                             m = cand2 - bias;
-                            ok = start2 - m >= kMinOffset && T.maybe(tag2, tag8((u32)v2)) && ld32(src + m) == (u32)v2;
+                            if constexpr (TT::kDict) ext_dict = T.ext && m < T.dend;
+                            if (ext_dict) {                    // :118-126
+                                if constexpr (TT::kDict) ok = start2 - m >= kMinOffset && T.dend - 1 - m >= 3 && ld32(T.dsrc + m) == (u32)v2;
+                            } else ok = start2 - m >= kMinOffset && T.maybe(tag2, tag8((u32)v2)) && ld32(src + m) == (u32)v2;
                         }
                         W::sync();
                         if (wr && (cand2 >= cur2 || cur2 >= cand2 + kMinOffset)) T.set_t(h2, cur2, tag8((u32)v2));   // lizard_parser_pricefast.h:190
                         W::sync();
                         if (ok) {
-                            const u32 mlt = count_match_par<W>(src + start2 + kMinMatch, src + m + kMinMatch, matchlimit) + kMinMatch;
+                            u32 mlt;
+                            if constexpr (TT::kDict) {
+                                if (ext_dict) mlt = count_2seg<W>(src + start2 + kMinMatch, T.dsrc + m + kMinMatch, matchlimit, T.dsrc + T.dend, src + T.dend) + kMinMatch;
+                                else mlt = count_match_par<W>(src + start2 + kMinMatch, src + m + kMinMatch, matchlimit) + kMinMatch;
+                            } else mlt = count_match_par<W>(src + start2 + kMinMatch, src + m + kMinMatch, matchlimit) + kMinMatch;
                             if (mlt >= min_match_long || start2 - m < kMax16BitOffset) { ml2 = mlt; ref2 = m; }
                         }
                     }
                     if (!ml2) break;
-                    {   const u32 back = extend_back_par<W>(src, start2, ref2, ip); start2 -= back; ref2 -= back; ml2 += back; }
+                    {
+                        u32 back;
+                        if constexpr (TT::kDict) back = dict_back<W>(T, src, start2, ref2, ip);
+                        else back = extend_back_par<W>(src, start2, ref2, ip);
+                        start2 -= back; ref2 -= back; ml2 += back;
+                    }
                     if (ml2 <= ml) { ml2 = 0; break; }
                     if (start2 <= ip) { ip = start2; ref = ref2; ml = ml2; ml2 = 0; break; }
                     if (start2 - ip < 3) { ip = start2; ref = ref2; ml = ml2; ml2 = 0; continue; }
@@ -1301,6 +1448,75 @@ template <class W> LZ_HD int encode_unit(const u8* src, u32 src_size, u8* dst, u
     case kEncFamFastBig: return encode_unit_fam<W, kEncFamFastBig>(src, src_size, dst, cap, level, T, work);
     default:             return encode_unit_fam<W, kEncFamGeneric>(src, src_size, dst, cap, level, T, work);
     }
+}
+
+// ---- compression against a loaded dictionary (hashChain and priceFast levels) ------------------------------------------------------
+// Lizard_loadDict's table (lizard_compress.c:426-437): Lizard_Insert over dictionary positions [0, upto) into a zero table and
+// the dictionary's chain (indexed by position & 0xFFFF; entries of positions the replay did not reach are never read: the
+// table and every chain delta only lead to inserted positions, or out of the window).
+template <class W> LZ_HD void dict_load(const u8* dict, u32 upto, const LevelParams& lp, u32* table, u16* chain)
+{
+    HashTable d; d.t32 = table; d.lo = nullptr; d.hi = nullptr; d.tag = nullptr; d.tagged = 0;
+    const PlainTable T(d);
+    T.template clear<W>(lp.hashLog);
+    ChainState cs = { chain, 0xFFFFu, 0, 0, lp.searchLength };
+    hc_insert<W, PlainTable>(dict, T, lp.hashLog, (1u << lp.windowLog) - 1, cs, upto);
+    W::sync();
+}
+// The parsers that search a loaded dictionary through the table Lizard_Insert fills (Lizard_hashPtr with the level's
+// searchLength): hashChain (13-17, 34-38) and priceFast (21, 22, 41, 42).
+LZ_HD bool dict_parser(const LevelParams& lp) { return lp.parser == kParserHashChain || lp.parser == kParserPriceFast; }
+// Lizard_compress_continue on a stream that Lizard_loadDict prepared (lizard_compress.c:550-580) at a dict_parser() level: returns
+// the compressed size or 0.  src is the parse's base (position 0 = the dictionary's first byte; the unit is at src + T.dend),
+// so for an external dictionary it is virtual and only positions >= T.dend are read through it.  One window runs across the
+// dictionary and every inner block of the unit.
+template <class W> LZ_HD int encode_unit_dict(const u8* src, u32 src_size, u8* dst, u32 cap, int level, const DictTable T,
+                                             EncWork* work)
+{
+    const LevelParams lp = level_params(level);
+    if (!dict_parser(lp)) return 0;
+    if (src_size > kMaxInputSize) return 0;
+    T.template clear<W>(lp.hashLog);
+    const bool wr = W::lane() == 0;
+    if (cap < 1) return 0;
+    if (wr) dst[0] = (u8)level;
+    long op = 1;
+    const long oend = (long)cap;
+    ParseCtx<DictTable> pc = { src, T, lp.hashLog, lp.windowLog };
+    ChainState cs = { work->chain, (1u << lp.chainLog) - 1, T.own0, lp.searchNum, lp.searchLength };
+    for (u32 pos = 0; pos < src_size;) {
+        const u32 part = src_size - pos < kBlockSize ? src_size - pos : kBlockSize;
+        const u32 b0 = T.dend + pos;
+        EncStreams s;
+        s.rec = work->seq; s.nseq = 0;
+        s.nl = s.nf = s.n16 = s.n24 = 0; s.tail_anchor = b0; s.tail_len = 0;
+        if (lp.parser == kParserHashChain) parse_hash_chain<W, DictTable>(pc, b0, b0 + part, s, cs);
+        else parse_price_fast_par<W, DictTable>(pc, b0, b0 + part, s, lp.minMatchLongOff);
+        W::sync();
+        if (write_block<W>(s, src, src + b0, part, dst, op, oend, lp.huffman != 0, lp.lizv1 != 0,
+                           work->lits, work->flags, &work->huf)) return 0;
+        W::sync();
+        pos += part;
+    }
+    return (int)op;
+}
+// The parse's view of one unit and its dictionary (dict_size already trimmed to the last kDictSize bytes): the layout, the
+// first position the unit inserts, and ctx->lowLimit after the overlap check of Lizard_compress_continue (:568-577).
+LZ_HD DictTable dict_view(const u8* unit, u32 unit_size, const u8* dict, u32 dict_size)
+{
+    DictTable T;
+    T.ov = nullptr; T.sh = nullptr; T.dchain = nullptr;
+    T.dsrc = dict; T.dend = dict_size;
+    T.ext = dict + dict_size != unit;
+    T.own0 = T.ext ? dict_size : (dict_size >= 8 ? dict_size - 7 : 0u);
+    u32 low = 0;
+    if (T.ext && unit + unit_size > dict && unit < dict + dict_size) {
+        const u8* e = unit + unit_size < dict + dict_size ? unit + unit_size : dict + dict_size;
+        low = (u32)(e - dict);
+        if (dict_size - low < 4) low = dict_size;
+    }
+    T.low = low + kDictSize;
+    return T;
 }
 
 }  // namespace lzb

@@ -10,6 +10,7 @@
 #define LZB_DICT_STATS 1          /* count the dictionary decoder's matches (lzb_dict_stats) */
 #define LZB_LP_STATS 1            /* count the lowestPrice parser's rare paths (lzb_lp_stats) */
 #define LZB_OPT_STATS 1           /* count the optimal parser's reference behaviours (lzb_opt_stats) */
+#define LZB_DICT_ENC_STATS 1      /* count priceFast matches that start in a dictionary (lzb_dict_enc_stats) */
 #include "entropy_dec.cuh"
 #include "encode_core.cuh"
 #include "encode_lp.cuh"
@@ -760,4 +761,56 @@ extern "C" int lzb_host_decompress2(const unsigned char* src, int csize, unsigne
     } else r = decode2_run<lzb::HostLanes>(src, csize, dst, cap, span, scratch, core, cs);
     free(scratch); free(core); free(cs);
     return r;
+}
+
+// ---- compression against a loaded dictionary (hashChain and priceFast levels) ------------------------------------------------------
+// Lizard_createStream(level) + Lizard_loadDict(dict, dict_size) + Lizard_compress_continue(src, dst, n, cap), one lane or the
+// 32-lane emulator: emu bit 0 runs the unit's parse on the emulator, bit 1 the dictionary's load too (the load is the
+// emulator's slowest part and the same code for every unit).  dict + dict_size == src is the prefix layout.
+// The device's scratch is not clean: the unit's chain and the loaded chain start as garbage, the overlay as garbage that the
+// unit clears.  Levels without a dictionary path return 0.
+unsigned long long lzb::g_dict_enc_stats[lzb::kDictEncStats];
+extern "C" void lzb_dict_enc_stats(unsigned long long* out, int reset)
+{
+    for (int k = 0; k < lzb::kDictEncStats; ++k) { if (out) out[k] = lzb::g_dict_enc_stats[k]; if (reset) lzb::g_dict_enc_stats[k] = 0; }
+}
+struct DictCompressArgs { const unsigned char* src; int n; unsigned char* dst; int cap; int level; const unsigned char* dict;
+                          lzb::u32 dsize; lzb::u32* ov; lzb::u32* sh; lzb::u16* dchain; lzb::EncWork* work; int emu_load; int result; };
+template <class W> static void dict_compress_body(DictCompressArgs* a)
+{
+    const lzb::LevelParams lp = lzb::level_params(a->level);
+    lzb::DictTable T = lzb::dict_view(a->src, (lzb::u32)a->n, a->dict, a->dsize);
+    if (a->emu_load || W::kLanes == 1) lzb::dict_load<W>(a->dict, a->dsize >= 8 ? a->dsize - 7 : 0u, lp, a->sh, a->dchain);
+    else if (W::lane() == 0) lzb::dict_load<lzb::HostLanes>(a->dict, a->dsize >= 8 ? a->dsize - 7 : 0u, lp, a->sh, a->dchain);
+    W::sync();
+    T.ov = a->ov; T.sh = a->sh; T.dchain = a->dchain;
+    const int r = lzb::encode_unit_dict<W>(a->src - a->dsize, (lzb::u32)a->n, a->dst, (lzb::u32)a->cap, a->level, T, a->work);
+    if (W::lane() == 0) a->result = r;
+}
+static void emu_dict_compress_body(void* p) { dict_compress_body<EmuLanes>((DictCompressArgs*)p); }
+
+extern "C" int lzb_dict_compress(const unsigned char* src, int n, unsigned char* dst, int cap, int level,
+                                 const unsigned char* dict, int dict_size, int emu)
+{
+    if (n < 0 || cap < 0 || dict_size < 0) return 0;
+    if (level > 49) level = 49;
+    if (level < 10) level = 17;
+    const lzb::LevelParams lp = lzb::level_params(level);
+    if (!lzb::dict_parser(lp)) return 0;
+    if (dict_size > (int)lzb::kDictSize) { dict += dict_size - (int)lzb::kDictSize; dict_size = (int)lzb::kDictSize; }   // :429-432
+    DictCompressArgs a;
+    a.src = src; a.n = n; a.dst = dst; a.cap = cap; a.level = level; a.dict = dict; a.dsize = (lzb::u32)dict_size; a.emu_load = emu & 2; a.result = 0;
+    a.ov = (lzb::u32*)malloc(sizeof(lzb::u32) << lp.hashLog);
+    a.sh = (lzb::u32*)malloc(sizeof(lzb::u32) << lp.hashLog);
+    a.dchain = (lzb::u16*)malloc(sizeof(lzb::u16) << 16);
+    a.work = (lzb::EncWork*)malloc(sizeof(lzb::EncWork));
+    a.work->huf.seg_count = (lzb::u32 (*)[256])malloc(4 * 256 * sizeof(lzb::u32));
+    memset(a.ov, 0x3C, sizeof(lzb::u32) << lp.hashLog);
+    memset(a.sh, 0x3C, sizeof(lzb::u32) << lp.hashLog);
+    memset(a.dchain, 0x5A, sizeof(lzb::u16) << 16);
+    memset(a.work->chain, 0xA5, sizeof a.work->chain);
+    if (emu & 1) emu::run(emu_dict_compress_body, &a);
+    else dict_compress_body<lzb::HostLanes>(&a);
+    free(a.work->huf.seg_count); free(a.work); free(a.dchain); free(a.sh); free(a.ov);
+    return a.result;
 }
