@@ -416,7 +416,34 @@ def _copy(out, off, n):
         out += (out[-off:] * (n // off + 1))[:n]
 
 
-def walk(comp, rep_short_at=None):
+def max_dist(level):
+    """The farthest offset a level's parser takes: 2^windowLog - 1 (64 KiB - 1 for the LZ4 codewords, 4 MiB - 1 for LIZv1
+    below level 29, whose window is 16 MiB)."""
+    if not is_lizv1(level):
+        return (1 << 16) - 1
+    return (1 << 24) - 1 if level in (29, 49) else (1 << 22) - 1
+
+
+class _DictCopy:
+    """Counts where a match's source lies when the output starts with a dictionary of `base` bytes."""
+
+    def __init__(self, out, classes, base, level):
+        self.out, self.classes, self.base, self.edge = out, classes, base, max_dist(level)
+
+    def __call__(self, off, n, kind):
+        src = len(self.out) - off
+        if self.base and 0 <= src < self.base:
+            kind_in = "dict_match" if src + n <= self.base else "dict_straddle"
+            self.classes[kind_in] += 1
+            self.classes[(kind_in, n)] += 1
+            if off == self.edge:
+                self.classes["dict_edge"] += 1
+            if kind:
+                self.classes["dict_" + kind] += 1
+        _copy(self.out, off, n)
+
+
+def walk(comp, rep_short_at=None, dictionary=b""):
     """Decode a Lizard stream whose inner blocks carry no Huffman-coded stream (levels 10-29, or blocks of the higher levels
     the encoder stored plain), following Lizard_decompress_generic (lib/lizard_decompress.c:115-264; streams as read by
     Lizard_readStream, :72-112).  Returns (decoded bytes, Counter of codeword classes):
@@ -427,7 +454,13 @@ def walk(comp, rep_short_at=None):
       rep_short                          a repeat-offset match of 2-3 bytes (LIZv1)
       raw_block, block                   stored and coded inner blocks
       ("lit", n), ("match", n), ("far", n)   lengths of literal runs, of 16-bit/repeat matches and of far matches.
-    If `rep_short_at` is a list, the output offset of every rep_short match is appended to it.
+    With a `dictionary` (a stream of Lizard_loadDict + Lizard_compress_continue) the output starts as the dictionary, matches
+    may reach into it, and the dictionary is stripped from the result.  Matches whose source starts in it also count as
+      dict_match, dict_straddle          the source lies wholly in the dictionary / runs on into the unit (also counted
+                                         by length: ("dict_match", n), ("dict_straddle", n))
+      dict_edge                          ... at offset max_dist(level), the farthest the window reaches
+      dict_far, dict_repeat              ... coded with a 24-bit offset / as a repeat offset (LIZv1).
+    If `rep_short_at` is a list, the unit offset of every rep_short match is appended to it.
     Raises ValueError on a stream the reference would refuse (as far as a valid-stream walker needs to tell)."""
     if not comp:
         raise ValueError("empty input")
@@ -435,8 +468,9 @@ def walk(comp, rep_short_at=None):
     if not 10 <= level <= 49:
         raise ValueError("level %d" % level)
     lizv1 = is_lizv1(level)
-    out = bytearray()
+    out = bytearray(dictionary)
     classes = Counter()
+    copy = _DictCopy(out, classes, len(dictionary), level)
     ip = 1
     while ip < len(comp):
         flag = comp[ip]
@@ -464,16 +498,16 @@ def walk(comp, rep_short_at=None):
         classes["block"] += 1
         _, off16, off24, flags, lits = (_Stream(s) for s in streams)
         if lizv1:
-            _block_liz(out, flags, lits, off16, off24, classes, rep_short_at)
+            _block_liz(out, flags, lits, off16, off24, classes, rep_short_at, copy)
         else:
-            _block_lz4(out, flags, lits, off16, off24, classes)
+            _block_lz4(out, flags, lits, off16, off24, classes, copy)
         if lits.p != len(lits.b):                       # last literals: the rest of the stream
             n = len(lits.b) - lits.p
             out += lits.take(n)
-    return bytes(out), classes
+    return bytes(out[len(dictionary):]), classes
 
 
-def _block_lz4(out, flags, lits, off16, off24, classes):
+def _block_lz4(out, flags, lits, off16, off24, classes, copy):
     while flags.p < len(flags.b):
         token = flags.byte()
         n = token & 15
@@ -492,10 +526,10 @@ def _block_lz4(out, flags, lits, off16, off24, classes):
             classes["match_ext0"] += 1
         ml += MINMATCH
         classes[("match", ml)] += 1
-        _copy(out, off, ml)
+        copy(off, ml, None)
 
 
-def _block_liz(out, flags, lits, off16, off24, classes, rep_short_at):
+def _block_liz(out, flags, lits, off16, off24, classes, rep_short_at, copy):
     last_off = 0                                        # LIZARD_INIT_LAST_OFFSET, per inner block
     lit_only = False
     while flags.p < len(flags.b):
@@ -523,10 +557,10 @@ def _block_liz(out, flags, lits, off16, off24, classes, rep_short_at):
             if ml and token >> 7 and ml < MINMATCH:       # only lowestPrice writes these: a 2-3 byte repeat-offset match
                 classes["rep_short"] += 1
                 if rep_short_at is not None:
-                    rep_short_at.append(len(out))
+                    rep_short_at.append(len(out) - copy.base)
             if ml:
                 classes[("match", ml)] += 1
-                _copy(out, last_off, ml)
+                copy(last_off, ml, "repeat" if token >> 7 else None)
             continue
         if token < LAST_LONG_OFF:
             ml = token + MM_LONGOFF
@@ -540,7 +574,7 @@ def _block_liz(out, flags, lits, off16, off24, classes, rep_short_at):
         last_off = _le(off24.take(3), 0, 3)
         classes["off24"] += 1
         classes[("far", ml)] += 1
-        _copy(out, last_off, ml)
+        copy(last_off, ml, "far")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -587,3 +621,219 @@ def targets(family, lizv1):
 def missing(family, lizv1, classes):
     """The targets of a family that `classes` lacks, by name."""
     return sorted((t for t in targets(family, lizv1) if classes[t] == 0), key=str)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# dictionaries: inputs for Lizard_loadDict + Lizard_compress_continue (hashChain 13-17 / 34-38, priceFast 21, 22, 41, 42)
+# ---------------------------------------------------------------------------------------------------------------------
+DICT_ENCODE_LEVELS = [13, 14, 15, 16, 17, 21, 22, 34, 35, 36, 37, 38, 41, 42]
+DICT_WALKED_LEVELS = [lv for lv in DICT_ENCODE_LEVELS if lv < 30]
+HC_WINDOW, PF_WINDOW = (1 << 16) - 1, (1 << 22) - 1          # max_dist of hashChain and of priceFast
+
+
+class DictCase:
+    """One unit and its dictionary.  prefix: the dictionary lies directly in front of the unit (otherwise it is external).
+    before_dict / after_dict / before_unit: bytes a layout must put right around the dictionary and the unit (empty: any
+    filler).  A poisoned case chooses them so that reading past the dictionary's end or extending a match below the start of
+    the dictionary or of the unit finds a longer match than the reference does.
+    expect: per codeword flavour ("lz4", "lizv1"), the walk classes (with their least counts) that the case's streams must
+    hold, summed over the DICT_WALKED_LEVELS of that flavour (dict_missing)."""
+
+    def __init__(self, family, dictionary, unit, prefix, before_dict=b"", after_dict=b"", before_unit=b"", lz4=(), lizv1=()):
+        self.family, self.dictionary, self.unit, self.prefix = family, dictionary, unit, prefix
+        self.before_dict, self.after_dict, self.before_unit = before_dict, after_dict, before_unit
+        self.expect = {"lz4": Counter(dict(lz4)), "lizv1": Counter(dict(lizv1))}
+
+    def __repr__(self):
+        return "DictCase(%s, dict %d, unit %d, %s)" % (self.family, len(self.dictionary), len(self.unit),
+                                                       "prefix" if self.prefix else "external")
+
+
+def _fresh(rng, n, avoid=None):
+    """n random bytes whose first byte differs from `avoid` (so a match in front of them cannot grow into them)."""
+    b = bytearray(_random(rng, n))
+    if n and avoid is not None and b[0] == avoid:
+        b[0] ^= 0x5A
+    return bytes(b)
+
+
+def _nonzero(rng, n):
+    """n random bytes, none of them 0: pieces that a match cannot grow into the zero filler around them."""
+    return rng.integers(1, 256, n, dtype=np.uint8).tobytes()
+
+
+def _far_cases(rng, window):
+    """A dictionary of window + 64 bytes, random in its first 8 KiB and zero behind them (so no later position takes the
+    random positions' buckets), and units holding 64-byte pieces of it at offsets window - 1, window and window + 1 (the
+    last out of reach) from where they are copied, each between 24 fresh bytes (so the block compresses)."""
+    d = _random(rng, 8192) + bytes(window + 64 - 8192)
+    out = []
+    for prefix in (False, True):
+        u = bytearray(_random(rng, 200))
+        for k in range(8):
+            for off in (window - 1, window, window + 1):
+                p = len(u)
+                q = len(d) + p - off                    # the piece's place in the dictionary
+                piece = d[q:q + 64]
+                if u[-1] == d[q - 1]:
+                    u[-1] ^= 0x77
+                u += piece
+                u += _fresh(rng, 24, d[q + 64])
+        if window == HC_WINDOW:                         # LIZv1 codes the pieces at 65536 - 1 and 65536 with 16 / 24 bits
+            expect = dict(lz4={"dict_match": 16, "dict_edge": 8}, lizv1={"dict_match": 24, "dict_far": 8})
+        else:                                           # out of the LZ4 window
+            expect = dict(lizv1={"dict_match": 16, "dict_far": 16, "dict_edge": 8})
+        out.append(DictCase("far", d, bytes(u), prefix, **expect))
+    return out
+
+
+def _straddle_cases(rng):
+    """One match per unit that starts k bytes before the dictionary's end and runs L - k bytes into the unit: the unit
+    begins with those L - k bytes, zeros follow, then the copy, then 1000 zeros (so the block gains the 512 bytes
+    Lizard_writeBlock asks of a coded block, lib/lizard_compress.c:228, and the copy is exactly one
+    match of L bytes; the dictionary and the copied bytes hold no zero).
+      * every match length of the codeword thresholds below 64 KiB (LZ4_MATCHES, LIZ_MATCHES, the LZ4 token's 15 and 19),
+        300 bytes behind the unit's start: a 16-bit offset in both flavours;
+      * FAR_LENGTHS, 66000 bytes behind it: a 24-bit offset, which LIZv1 takes from 20 bytes on (MM_LONGOFF + MINMATCH);
+        the shorter ones must stay literals;
+      * LIZ_MATCHES' 65550 and 65551, nearly all in the dictionary, more than 64 KiB back: LIZv1 only.
+    The LZ4 lengths of 64 KiB and more cannot straddle: such a match would reach further back than the 64 KiB window."""
+    d = _nonzero(rng, 70000)
+    near = sorted(L for L in set(LZ4_MATCHES + LIZ_MATCHES + (15, 19)) if L < 60000)
+    jobs = [(L, 300, "both") for L in near] + [(L, 66000, "lizv1" if L >= MM_LONGOFF + MINMATCH else "none")
+                                                for L in FAR_LENGTHS] + [(L, 100, "lizv1") for L in (65550, 65551)]
+    out = []
+    for j, (L, gap, flavours) in enumerate(jobs):
+        k = L - 40 if L > 60000 else (8, 12, 9, 33)[j % 4] if L > 33 else 8
+        head = _nonzero(rng, L - k + 1)                 # the match runs over head[:L - k]; head[L - k] ends the source
+        u = head + bytes(gap) + d[-k:] + head[:L - k] + bytes(1000)
+        want = {("dict_straddle", L): 1}
+        expect = {"both": dict(lz4=want, lizv1=want), "lizv1": dict(lizv1=want), "none": {}}[flavours]
+        out.append(DictCase("straddle", d, u, j % 2 == 1, **expect))
+    return out
+
+
+def _periodic_cases(rng):
+    """Dictionaries that repeat a period of 1-8, 16 or 33 bytes (same-bucket runs inside one 32-position load step), with a
+    changed byte now and then, and units made of pieces of them and fresh bytes."""
+    out = []
+    for i, p in enumerate((1, 2, 3, 4, 5, 6, 7, 8, 16, 33)):
+        base = bytearray((_random(rng, p) * (6000 // p + 1))[:6000])
+        for at in rng.integers(100, len(base), size=3):
+            base[int(at)] ^= 0xA5
+        d = _random(rng, 700) + bytes(base) + _random(rng, 300)
+        u = d[900:2500] + _random(rng, 500) + d[-400:] + bytes(base[:300]) + _random(rng, 100)
+        out.append(DictCase("periodic", d, u, i % 2 == 0, lz4={"dict_match": 1}, lizv1={"dict_match": 1}))
+    return out
+
+
+def _tiny_cases(rng):
+    """Dictionaries of 0 to 8 bytes, both layouts: the unit repeats the dictionary's bytes between zero runs, so its block
+    is coded (its zeros pay for the 512 bytes a coded block must gain)."""
+    out = []
+    for n in range(9):
+        d = _random(rng, n)
+        u = d + bytes(30) + d * 3 + _random(rng, 50) + bytes(1200) + (d + b"xyz") * 4
+        out += [DictCase("tiny", d, u, prefix, lz4={"block": 1}, lizv1={"block": 1}) for prefix in (False, True)]
+    return out
+
+
+def _repeat_cases(rng):
+    """Pieces of the dictionary with one byte changed every 40: each piece after the first continues at the previous
+    match's offset (a LIZv1 repeat offset into the dictionary)."""
+    d = _random(rng, 30000)
+    out = []
+    for prefix in (False, True):
+        piece = bytearray(d[20000:26000])
+        for k in range(0, len(piece), 40):
+            piece[k] ^= 0x55
+        u = _random(rng, 500) + bytes(piece) + _random(rng, 2000) + d[-300:] + b"#" + d[-200:]
+        out.append(DictCase("repeat", d, u, prefix, lz4={"dict_match": 100}, lizv1={"dict_match": 100, "dict_repeat": 100}))
+    return out
+
+
+def _corpus_cases():
+    """Every corpus unit, cut to 64 KiB, against a dictionary of 32 KiB of another corpus unit and the unit's own last
+    32 KiB (for a unit of more than 64 KiB, bytes that follow the cut, of the same kind)."""
+    units = corpus_units()
+    out = []
+    for i, u in enumerate(units):
+        d = units[(i + 7) % len(units)][-32768:] + u[-32768:]
+        out.append(DictCase("corpus", d, u[:65536], i % 3 == 0))
+    return out
+
+
+def _poisoned_cases(rng):
+    """A dictionary A + M + B (A, B of 24 bytes) and a unit C 0... Y A 0... B X 0... whose first 24 bytes C are a piece of
+    M; between them zero runs, so the block is coded and A, B and C are dictionary matches of exactly 24 bytes (the
+    pieces hold no zero).  The bytes after the dictionary are X (what follows B in the unit), the bytes in front of the
+    dictionary are Y (what precedes A in the unit) and the bytes in front of the unit are those in front of C in M.  A
+    kernel that counts on in the dictionary's buffer past its end instead of at the unit's first byte, or extends a match
+    below the dictionary's or the unit's start, finds longer matches than the reference."""
+    out = []
+    for j in range(4):
+        A, B, M = _nonzero(rng, 24), _nonzero(rng, 24), _nonzero(rng, 3000)
+        d = A + M + B
+        c_at = 1000 + 100 * j
+        C = M[c_at:c_at + 24]
+        X, Y = bytearray(_nonzero(rng, 40)), _nonzero(rng, 32)
+        if X[0] == C[0]:                                # B's match continues at the unit's first byte, and stops there
+            X[0] ^= 0x5A
+        u = C + bytes(400) + Y + A + bytes(300) + B + bytes(X) + bytes(300)
+        prefix = j == 3
+        want = {("dict_match", 24): 2}                  # A and B; C's match starts behind the unit's first byte, a literal
+        out.append(DictCase("poisoned", d, u, prefix, before_dict=Y, after_dict=b"" if prefix else bytes(X),
+                            before_unit=b"" if prefix else M[c_at - 32:c_at], lz4=want, lizv1=want))
+    return out
+
+
+def dict_corpus(seed=90):
+    """The dictionary cases, family by family (far, straddle, periodic, tiny, repeat, corpus, poisoned); seeded, about
+    12 MiB of dictionaries (the two 4 MiB ones twice) and 2.6 MiB of units."""
+    rng = np.random.default_rng(seed)
+    return (_far_cases(rng, HC_WINDOW) + _far_cases(rng, PF_WINDOW) + _straddle_cases(rng) + _periodic_cases(rng)
+            + _tiny_cases(rng) + _repeat_cases(rng) + _corpus_cases() + _poisoned_cases(rng))
+
+
+def dict_targets():
+    """Codeword classes the streams of dict_corpus() reach, summed over DICT_WALKED_LEVELS: matches from the dictionary, into
+    the unit, at the window's last offset, and (LIZv1) with 24-bit and repeat offsets into the dictionary."""
+    return {"dict_match", "dict_straddle", "dict_edge", "dict_far", "dict_repeat"}
+
+
+def poisoned_parse_ok(classes):
+    """A poisoned unit's stream at one level: three dictionary matches (C, A, B) of 23 or 24 bytes and none longer, which a
+    kernel that read the poisoned surroundings would have found."""
+    lengths = Counter({k[1]: v for k, v in classes.items() if isinstance(k, tuple) and k[0] == "dict_match"})
+    return sum(lengths.values()) == 3 and set(lengths) <= {23, 24}
+
+
+def dict_missing(case, lizv1, classes):
+    """What `classes` (summed over the case's walked levels of one flavour) lacks of case.expect: (class, have, want)."""
+    want = case.expect["lizv1" if lizv1 else "lz4"]
+    return sorted(((k, classes[k], n) for k, n in want.items() if classes[k] < n), key=str)
+
+
+CORPUS_DICT_SHARE = 0.5         # the least share of the corpus family's cases whose streams hold a dictionary match
+
+
+def dict_shortfalls(cases, walked):
+    """walked: level -> the walk classes of every case at that level (DICT_WALKED_LEVELS).  Returns what falls short, case
+    by case and flavour by flavour: the expectations of dict_missing, and for the corpus family the share of cases with a
+    dictionary match (CORPUS_DICT_SHARE).  Empty when every family reaches what it is built for."""
+    out = []
+    for lizv1 in (False, True):
+        seen = [Counter() for _ in cases]
+        for level, per_case in walked.items():
+            if is_lizv1(level) == lizv1:
+                for acc, classes in zip(seen, per_case):
+                    acc.update(classes)
+        for i, (c, acc) in enumerate(zip(cases, seen)):
+            m = dict_missing(c, lizv1, acc)
+            if m:
+                out.append((i, c, "lizv1" if lizv1 else "lz4", m))
+        corp = [acc for c, acc in zip(cases, seen) if c.family == "corpus"]
+        share = sum(1 for acc in corp if acc["dict_match"]) / max(len(corp), 1)
+        if share < CORPUS_DICT_SHARE:
+            out.append(("corpus", "lizv1" if lizv1 else "lz4", share))
+    return out

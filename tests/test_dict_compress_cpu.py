@@ -4,11 +4,14 @@ encoder's code on the CPU: the one-lane host build and the 32-lane warp emulator
 against the compiled reference, byte for byte and with the same return value.  Both layouts count: the dictionary directly
 in front of the input (prefix) and a dictionary somewhere else (external)."""
 import ctypes
+import functools
 import os
+import random
+from collections import Counter
 
 import pytest
 
-from tests import refs
+from tests import corpus, refs
 from tests.test_dict_cpu import _dictionary, _straddler, records
 
 HC_LEVELS = list(range(13, 18)) + list(range(34, 39))
@@ -17,11 +20,7 @@ DICT_LEVELS = HC_LEVELS + PF_LEVELS
 DICT_LIMIT = 1 << 24
 
 
-@pytest.fixture(scope="module")
-def ref():
-    L = refs.ref_parity()
-    if L is None:
-        pytest.skip("oracle/_ref not built")
+def _bind_stream(L):
     vp, ci = ctypes.c_void_p, ctypes.c_int
     L.Lizard_createStream.restype = vp
     L.Lizard_createStream.argtypes = [ci]
@@ -29,6 +28,18 @@ def ref():
     L.Lizard_loadDict.argtypes = [vp, vp, ci]
     L.Lizard_compress_continue.argtypes = [vp, vp, vp, ci, ci]
     return L
+
+
+def lz_bound(n):
+    return n + 2 + (n // (1 << 17) + 1) * 4
+
+
+@pytest.fixture(scope="module")
+def ref():
+    L = refs.ref_parity()
+    if L is None:
+        pytest.skip("oracle/_ref not built")
+    return _bind_stream(L)
 
 
 @pytest.fixture(scope="module")
@@ -72,7 +83,7 @@ def dev_run(shim, level, dict_p, dict_n, src_p, n, cap, emu):
 
 def check(ref, shim, level, dictionary, data, prefix, caps=None, orders=(0, 1, 2), emu=1):
     keep, dict_p, src_p = _layout(dictionary, data, prefix)
-    bound = len(data) + 2 + (len(data) // (1 << 17) + 1) * 4
+    bound = lz_bound(len(data))
     want_full = ref_run(ref, level, dict_p, len(dictionary), src_p, len(data), bound)
     caps = caps if caps is not None else [bound]
     for cap in caps:
@@ -232,3 +243,101 @@ def test_dictionary_encode_kernel_resources():
             res = {k: int(v) for k, v in re.findall(r"(REG|STACK|LOCAL|SHARED):(\d+)", line)}
             name = None
     assert res == DICT_ENCODE_KERNEL, res
+
+
+# ---- the dictionary corpus (tests/corpus.py dict_corpus) ----------------------------------------------------------------
+@functools.lru_cache(maxsize=None)
+def _dict_corpus():
+    return corpus.dict_corpus()
+
+
+@functools.lru_cache(maxsize=None)
+def _ref_dict_streams(level):
+    L = refs.ref_parity()
+    _bind_stream(L)
+    out = []
+    for c in _dict_corpus():
+        keep, dict_p, src_p = _layout(c.dictionary, c.unit, c.prefix)
+        out.append(ref_run(L, level, dict_p, len(c.dictionary), src_p, len(c.unit), lz_bound(len(c.unit)))[1])
+        del keep
+    return out
+
+
+@pytest.mark.parametrize("level", corpus.DICT_WALKED_LEVELS)
+def test_walker_decodes_reference_dictionary_streams(ref, level):
+    """The walker, given the dictionary, decodes the reference's dictionary streams to the input; without it, a stream that
+    reaches into the dictionary is refused."""
+    refused = 0
+    for c, comp in zip(_dict_corpus(), _ref_dict_streams(level)):
+        out, classes = corpus.walk(comp, dictionary=c.dictionary)
+        assert out == c.unit, (level, c)
+        if classes["dict_match"] + classes["dict_straddle"]:
+            with pytest.raises(ValueError):
+                corpus.walk(comp)
+            refused += 1
+    assert refused > 10, level
+
+
+def test_reference_dictionary_streams_reach_every_target(ref):
+    """Case by case, the reference's streams hold what each family is built for (corpus.dict_shortfalls: a coded block, the
+    straddle of exactly its length, the three 24-byte matches of a poisoned unit, the window's last offset at both window
+    sizes, ...), and all of them together every class of corpus.dict_targets()."""
+    walked = {level: [corpus.walk(comp, dictionary=c.dictionary)[1] for c, comp in zip(_dict_corpus(), _ref_dict_streams(level))]
+              for level in corpus.DICT_WALKED_LEVELS}
+    short = corpus.dict_shortfalls(_dict_corpus(), walked)
+    short += [(level, i) for level, per_case in walked.items() for i, (c, classes) in enumerate(zip(_dict_corpus(), per_case))
+              if c.family == "poisoned" and not corpus.poisoned_parse_ok(classes)]
+    assert not short, short[:10]
+    seen = Counter()
+    for per_case in walked.values():
+        for classes in per_case:
+            seen.update(classes)
+    assert not [t for t in corpus.dict_targets() if seen[t] == 0], dict(seen)
+
+
+@pytest.mark.parametrize("level", corpus.DICT_WALKED_LEVELS)
+def test_poisoned_surroundings_change_the_reference_output(ref, level):
+    """The bytes a poisoned case puts around its dictionary matter: the reference given them as part of the dictionary (what
+    a kernel reading past the dictionary's end, or extending below its start, would see) writes a different stream.  So a
+    device call that writes the reference's bytes with those surroundings in place did not read them."""
+    for c in _dict_corpus():
+        if c.family != "poisoned":
+            continue
+        want = _ref_stream(ref, level, c.dictionary, c.unit, c.prefix)
+        assert _ref_stream(ref, level, c.before_dict + c.dictionary, c.unit, c.prefix) != want, (level, c, "before")
+        if c.after_dict:
+            assert _ref_stream(ref, level, c.dictionary + c.after_dict, c.unit, False) != want, (level, c, "after")
+
+
+def _ref_stream(ref, level, dictionary, unit, prefix):
+    keep, dict_p, src_p = _layout(dictionary, unit, prefix)
+    r = ref_run(ref, level, dict_p, len(dictionary), src_p, len(unit), lz_bound(len(unit)))
+    del keep
+    return r
+
+
+def _emulated(cases, level):
+    """What the coroutine emulator (slow) runs: every case but the corpus family's, whose first two it runs cut to 20000
+    bytes; at the hashChain levels (the slowest under the emulator) the first two cases of each family, cut to 20000."""
+    out, seen = [], Counter()
+    for c in cases:
+        if c.family == "corpus" or level in HC_LEVELS:
+            if seen[c.family] < 2:
+                out.append((c, c.unit[:20000]))
+            seen[c.family] += 1
+        else:
+            out.append((c, c.unit))
+    return out
+
+
+@pytest.mark.parametrize("level", DICT_LEVELS)
+def test_dict_families_one_lane_and_emulated_bit_exact(ref, shim, level):
+    """Every family of the dictionary corpus through the one-lane host build at every level with a dictionary path, at the
+    bound and at an edge capacity, and the emulator in lane order 0 (_emulated): the reference's bytes and return value."""
+    rnd = random.Random(700 + level)
+    cases = _dict_corpus()
+    caps = corpus.edge_capacities(rnd, [c.unit for c in cases], lz_bound)
+    for c, cap in zip(cases, caps):
+        check(ref, shim, level, c.dictionary, c.unit, c.prefix, caps=[lz_bound(len(c.unit)), cap], orders=())
+    for c, unit in _emulated(cases, level):
+        check(ref, shim, level, c.dictionary, unit, c.prefix, orders=(0,))
