@@ -252,13 +252,16 @@ def test_reach_edges(ref, shim, level):
                 assert r < -1, (k, need, r)                     # a token error, not the header / stream error -1
 
 
-def _long_offset_unit(level, off, ml_code=5):
+def _long_offset_unit(level, off, ml_code=5, lead=0):
     """A LIZv1 unit of one inner block, all streams raw: one 24-bit-offset token (match length ml_code + 16) at the unit start,
-    then 16 literals.  Its match starts `off` bytes below the unit start."""
+    then 16 literals.  Its match starts `off` bytes below the unit start.  lead = 1..7: in front of it a token of `lead`
+    literals and an 8-byte match at 16-bit offset 1000, so the far match starts off - lead - 8 bytes below the unit start."""
     le24 = lambda v: bytes([v & 255, (v >> 8) & 255, v >> 16])
-    lits = bytes(range(65, 81))
-    body = le24(0) + le24(0) + le24(3) + le24(off) + le24(1) + bytes([ml_code]) + le24(len(lits)) + lits
-    return bytes([level, 0]) + body, ml_code + 16 + len(lits)
+    lits = bytes(range(65 - lead, 81))
+    off16 = bytes([1000 & 255, 1000 >> 8]) if lead else b""
+    flags = (bytes([(8 << 3) | lead]) if lead else b"") + bytes([ml_code])
+    body = (le24(0) + le24(len(off16)) + off16 + le24(3) + le24(off) + le24(len(flags)) + flags + le24(len(lits)) + lits)
+    return bytes([level, 0]) + body, (lead + 8 if lead else 0) + ml_code + 16 + 16
 
 
 @pytest.mark.parametrize("prefix", [True, False])
@@ -284,10 +287,14 @@ def test_the_2_24_switches(ref, shim, prefix):
     assert dev_decode_dict(shim, HOST, comp, d, len(data), prefix, avail=65535)[1] == data
 
 
-def _linked_stream(ref, data, level, piece, double_buffer):
+def _linked_stream(ref, data, level, piece, double_buffer, place=None, load=None):
     """The reference's streamed compression: Lizard_compress_continue on consecutive pieces of one buffer, or on pieces
-    copied into two buffers in turn (each piece then sees only the one before it, lizard_compress.c:439-449)."""
+    copied into two buffers in turn (each piece then sees only the one before it, lizard_compress.c:439-449), or on pieces
+    copied to the addresses place(k) that the caller chooses (so the compressor sees the layout a decoder will use).
+    load = (address, size): Lizard_loadDict of those bytes first."""
     st = ref.Lizard_createStream(level)
+    if load:
+        ref.Lizard_loadDict(st, load[0], load[1])
     src = ctypes.create_string_buffer(data, len(data) + 1)
     two = [ctypes.create_string_buffer(piece + 1) for _ in range(2)]
     out = []
@@ -296,8 +303,8 @@ def _linked_stream(ref, data, level, piece, double_buffer):
         cap = n_in + n_in // 8 + 1024
         buf = ctypes.create_string_buffer(cap)
         where = ctypes.addressof(src) + at
-        if double_buffer:
-            where = ctypes.addressof(two[(at // piece) % 2])
+        if double_buffer or place:
+            where = place(at // piece) if place else ctypes.addressof(two[(at // piece) % 2])
             ctypes.memmove(where, data[at:at + n_in], n_in)
         n = ref.Lizard_compress_continue(st, where, buf, n_in, cap)
         assert n > 0
