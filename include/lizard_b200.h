@@ -274,6 +274,38 @@ int LizardB200_compress_dict_device(const void* dSrc, const uint64_t* dSrcOff, c
  * packs the units of a batch back to back.  Enqueue-only, like the calls above. */
 int LizardB200_gather_device(const void* dSrc, const uint64_t* dSrcOff, const int* dLen,
                              void* dDst, const uint64_t* dDstOff, unsigned nUnits, void* cudaStream);
+/* LizardF frames in device memory (DESIGN.md 3.4a).  Payload in DEVICE memory of the current device: frame i is the srcSize[i]
+ * bytes at dSrc + srcOff[i] and goes to dDst + dstOff[i] with room for dstCap[i] bytes.  Tables and results are in HOST memory.
+ * Unlike the enqueue-only calls above these SYNCHRONISE `cudaStream` and return when their work is done: where a frame's blocks
+ * lie, and which verdict a frame gets, is only known once its headers and block results have been read back from the device.
+ * Same workspace and stream rules as the calls above.  Nothing is written outside [dDst + dstOff[i], dDst + dstOff[i] + dstCap[i]).
+ * The return value is LIZARDB200_OK or a negative batch status; result[i] is a size_t that LizardF_isError tests.
+ *
+ * LizardB200_compressFrames: frame i equals LizardF_compressFrame(dst, dstCap[i], src, srcSize[i], prefs) of this library on host
+ * copies, byte for byte and in its return value (errors included, when nothing is written).  One difference, where the host call
+ * writes past dstMaxSize: a 1-byte input whose header carries the content size, given 25 to 28 bytes of room (25 to 32 with the
+ * content checksum; LizardF_compressFrameBound says 24 / 28), gets LizardF_ERROR_dstMaxSize_tooSmall here.  Its 1-byte block
+ * takes 10 bytes, 5 more than the bound counts.  A fixed number of launches however many frames: one encode launch over every block of every frame, then the content
+ * checksums and the frame assembly.
+ *
+ * LizardB200_decompressFrames: result[i] is what LizardF_decompress on a fresh context returns for frame i handed its whole
+ * srcSize[i] bytes and dstCap[i] bytes of room in one call: the decoded size if that call finishes the frame, the same error code
+ * if it fails; LizardF_ERROR_frameSize_wrong if it would end having read all input without finishing the frame (a truncated
+ * frame) or finish it with input left (more bytes behind the frame); LizardF_ERROR_dstMaxSize_tooSmall if it would stop because
+ * the output is full, with input left; 0 for a skippable
+ * frame (nothing written); LizardF_ERROR_blockMode_invalid for a linked frame.  Damage in one frame changes no other frame's
+ * result or bytes; after an error the frame's own dst range holds unspecified bytes.  The decoder stages every compressed block
+ * in a workspace slot of its frame's maximum block size, at most 4 GiB of slots at a time: frames of many blocks far smaller
+ * than their maximum take several decode rounds (more launches), never a failure of the call.  LIZARDB200_ERR_MEMORY only when
+ * the device cannot hold one slot of the call's largest maximum block size.
+ * The content checksum of one frame is computed by one warp (about 1.2 GB/s on an H100): for a single large checksummed frame
+ * the host frame API, which hashes on a host thread, is faster. */
+int LizardB200_compressFrames(const void* dSrc, const uint64_t* srcOff, const uint64_t* srcSize,
+                              void* dDst, const uint64_t* dstOff, const uint64_t* dstCap,
+                              size_t* result, unsigned nFrames, const LizardF_preferences_t* prefs, void* cudaStream);
+int LizardB200_decompressFrames(const void* dSrc, const uint64_t* srcOff, const uint64_t* srcSize,
+                                void* dDst, const uint64_t* dstOff, const uint64_t* dstCap,
+                                size_t* result, unsigned nFrames, void* cudaStream);
 /* diagnostics: launch shape of the encode kernel for a level (no device needed): warps per CTA, how many of them keep their
  * hash table in shared memory, CTAs per SM (an upper bound: a launch holds no more than fit), dynamic shared memory per CTA.
  * The level's default, or LIZARDB200_ENC_SHAPE="warps,tables,ctas" when that is set and valid, exactly as the encoder

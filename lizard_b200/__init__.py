@@ -69,6 +69,14 @@ def lib():
                                                  ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
         L.LizardB200_decompress_blocks.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
                                                    ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+        u64p = ctypes.POINTER(ctypes.c_uint64)
+        L.LizardB200_compressFrames.argtypes = [ctypes.c_void_p, u64p, u64p, ctypes.c_void_p, u64p, u64p,
+                                                ctypes.POINTER(ctypes.c_size_t), ctypes.c_uint, ctypes.c_void_p, ctypes.c_void_p]
+        L.LizardB200_decompressFrames.argtypes = [ctypes.c_void_p, u64p, u64p, ctypes.c_void_p, u64p, u64p,
+                                                  ctypes.POINTER(ctypes.c_size_t), ctypes.c_uint, ctypes.c_void_p]
+        L.LizardF_isError.argtypes = [ctypes.c_size_t]
+        L.LizardF_getErrorName.argtypes = [ctypes.c_size_t]
+        L.LizardF_getErrorName.restype = ctypes.c_char_p
         _lib = L
     return _lib
 
@@ -344,3 +352,41 @@ def frame_decompress(L, frame: bytes, out_cap: int, chunk: int = 0, dst_chunk: i
     finally:
         L.LizardF_freeDecompressionContext(ctx)
     return res, out.raw[:op]
+
+
+# ---- LizardF frames in device memory (LizardB200_compressFrames / LizardB200_decompressFrames) -----------------------
+def _frame_tables(src_off, src_size, dst_off, dst_cap):
+    n = len(src_off)
+    if not (len(src_size) == len(dst_off) == len(dst_cap) == n):
+        raise ValueError("one offset, size, destination offset and capacity per frame")
+    u64 = ctypes.c_uint64 * n
+    return n, u64(*src_off), u64(*src_size), u64(*dst_off), u64(*dst_cap), (ctypes.c_size_t * n)()
+
+
+def compress_frames(d_src: int, src_off, src_size, d_dst: int, dst_off, dst_cap, prefs, stream: int = 0):
+    """LizardB200_compressFrames: frame i is LizardF_compressFrame of the src_size[i] bytes at device address d_src + src_off[i],
+    written to d_dst + dst_off[i] with room for dst_cap[i] bytes.  Addresses are integers (e.g. a tensor's data_ptr()), the
+    tables host lists; `stream` is a cudaStream_t as an integer (0 = the default stream).  The call synchronises that stream.
+    Returns the per-frame results (size_t: the frame size, or a LizardF error code, see frame_error)."""
+    L = lib()
+    n, so, ss, do, dc, res = _frame_tables(src_off, src_size, dst_off, dst_cap)
+    _check(L.LizardB200_compressFrames(d_src, so, ss, d_dst, do, dc, res, n, ctypes.byref(prefs), stream or None),
+           "LizardB200_compressFrames")
+    return list(res)
+
+
+def decompress_frames(d_src: int, src_off, src_size, d_dst: int, dst_off, dst_cap, stream: int = 0):
+    """LizardB200_decompressFrames: frame i is the src_size[i] bytes at d_src + src_off[i], decoded to d_dst + dst_off[i] with
+    room for dst_cap[i] bytes, as LizardF_decompress would in one call given all of it (include/lizard_b200.h).  Same argument
+    conventions as compress_frames.  Returns the per-frame results (size_t: decoded size, 0 for a skippable frame, or a
+    LizardF error code)."""
+    L = lib()
+    n, so, ss, do, dc, res = _frame_tables(src_off, src_size, dst_off, dst_cap)
+    _check(L.LizardB200_decompressFrames(d_src, so, ss, d_dst, do, dc, res, n, stream or None), "LizardB200_decompressFrames")
+    return list(res)
+
+
+def frame_error(result: int):
+    """None if a frame result is a size, else its LizardF error name (e.g. "ERROR_frameSize_wrong")."""
+    L = lib()
+    return L.LizardF_getErrorName(result).decode() if L.LizardF_isError(result) else None

@@ -8,6 +8,7 @@
 #include "encode_lp_kernel.cuh"
 #include "encode_opt_kernel.cuh"
 #include "encode_dict_kernel.cuh"
+#include "frame_device_kernels.cuh"
 
 #include <cuda_runtime.h>
 #include <mutex>
@@ -230,6 +231,7 @@ struct Context {
     PinnedBuffer pin_in, pin_out, pin_tab, pin_flags;
     DeviceBuffer d_progress;
     DeviceBuffer d_in, d_out, d_tab, d_pack;
+    DeviceBuffer fd_tab, fd_stage;            // tables and staged blocks of the device-memory frame calls (frame.inl)
     EncodeConfig enc_cfg;
 };
 Context g_ctx[kMaxDevices];

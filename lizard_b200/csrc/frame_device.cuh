@@ -1,0 +1,222 @@
+// frame_device.cuh -- LizardF frames held in device memory (LizardB200_compressFrames / LizardB200_decompressFrames,
+// DESIGN.md 3.4a): the XXH32 routine, the header check and block walk of one frame, and the kernels that run them over
+// many frames at once.  XXH32 and the walk are plain serial code that the host shim builds too (host_shim.cpp), so the
+// CPU tests pin them against the reference's xxhash.c and frame layer; the kernels are device-only.
+//
+// Reference: lib/xxhash/xxhash.c (XXH32), lib/lizard_frame.c:756-857 (header), :980-1320 (block loop), format
+// doc/lizard_Frame_format.md.
+#pragma once
+#include "common.cuh"
+
+namespace lzb {
+
+// ---- XXH32 (public algorithm) --------------------------------------------------------------------------------------
+constexpr u32 kXxP1 = 2654435761u, kXxP2 = 2246822519u, kXxP3 = 3266489917u, kXxP4 = 668265263u, kXxP5 = 374761393u;
+LZ_HD u32 xx_rotl(u32 v, int r) { return (v << r) | (v >> (32 - r)); }
+LZ_HD u32 xx_round(u32 acc, u32 in) { return xx_rotl(acc + in * kXxP2, 13) * kXxP1; }
+LZ_HD u32 xx_lane_init(u32 seed, u32 lane)
+{
+    return lane == 0 ? seed + kXxP1 + kXxP2 : lane == 1 ? seed + kXxP2 : lane == 2 ? seed : seed - kXxP1;
+}
+// the digest from the four lane accumulators (ignored below 16 bytes), the length and the last n % 16 bytes
+LZ_HD u32 xx_finish(const u32 v[4], u64 total, const u8* tail, u32 ntail, u32 seed)
+{
+    u32 h = total >= 16 ? xx_rotl(v[0], 1) + xx_rotl(v[1], 7) + xx_rotl(v[2], 12) + xx_rotl(v[3], 18) : seed + kXxP5;
+    h += (u32)total;
+    u32 i = 0;
+    for (; i + 4 <= ntail; i += 4) h = xx_rotl(h + rd_le32(tail + i) * kXxP3, 17) * kXxP4;
+    for (; i < ntail; ++i) h = xx_rotl(h + tail[i] * kXxP5, 11) * kXxP1;
+    h ^= h >> 15; h *= kXxP2; h ^= h >> 13; h *= kXxP3; h ^= h >> 16;
+    return h;
+}
+// one thread, one buffer: the header checksum byte, and the host build's content checksum
+LZ_HD u32 xxh32_serial(const u8* p, u64 n, u32 seed)
+{
+    u32 v[4] = { xx_lane_init(seed, 0), xx_lane_init(seed, 1), xx_lane_init(seed, 2), xx_lane_init(seed, 3) };
+    const u64 stripes = n / 16;
+    for (u64 s = 0; s < stripes; ++s)
+        for (int l = 0; l < 4; ++l) v[l] = xx_round(v[l], rd_le32(p + 16 * s + 4 * l));
+    return xx_finish(v, n, p + 16 * stripes, (u32)(n % 16), seed);
+}
+
+// ---- one frame's header and block chain ------------------------------------------------------------------------------
+// Verdicts use the numbering of LizardF_errorCodes (lib/lizard_frame_static.h:56-67); frame.inl ties them to its own.
+enum : u32 { kFwOk = 0, kFwGeneric = 1, kFwMaxBlockSize = 2, kFwBlockMode = 3, kFwHeaderVersion = 6, kFwBlockChecksum = 7,
+             kFwReserved = 8, kFwDstTooSmall = 11, kFwFrameType = 13, kFwFrameSize = 14, kFwDecompressionFailed = 16,
+             kFwHeaderChecksum = 17, kFwContentChecksum = 18 };
+// How the bytes after the last complete block end (FrameInfoRec::tail)
+enum : u32 { kTailEnd = 0,          // end mark, checksum if flagged, nothing behind
+             kTailTrailing = 1,     // the same, followed by more bytes
+             kTailTruncated = 2,    // the bytes stop inside a block header, a block or the checksum
+             kTailGeneric = 3,      // a block header announces more than the maximum block size
+             kTailSkippable = 4 };  // a complete skippable frame (trailing bytes give kTailTrailing with skippable = 1)
+struct FrameInfoRec {
+    u32 verdict;          // kFwOk, or the header's error (then nothing else is set)
+    u32 tail;             // kTail*
+    u32 skippable;
+    u32 ccksum;           // content checksum flag
+    u32 stored_cksum;     // the frame's content checksum word (tail == kTailEnd / kTailTrailing with ccksum)
+    u32 max_block;
+    u32 n_blocks;         // complete blocks in front of the tail (a truncated block is not counted)
+    u32 trunc_block;      // tail kTailTruncated inside a block: 1 compressed, 2 raw (0: inside a header word or the checksum)
+    u64 trunc_avail;      // the bytes of that block present
+    u64 content_size;     // 0 = not given
+};
+struct FrameBlockRec {
+    u64 src;              // offset of the payload from the frame's first byte
+    u32 csize;            // payload bytes
+    u32 raw;              // 1 = stored block
+};
+
+// maximum block size of a block size ID (lib/lizard_frame.c:194), 0 for an invalid one; frame.inl's frame_block_size too
+LZ_HD u32 frame_block_bytes(u32 bsid)
+{
+    return bsid == 1 ? 128u << 10 : bsid == 2 ? 256u << 10 : bsid >= 3 && bsid <= 7 ? 1u << (20 + 2 * (bsid - 3)) : 0u;
+}
+
+// Header check and block walk of the n bytes at p, as LizardF_decompress (frame.inl) sees them when handed all n bytes at
+// once; blocks (if not null) gets the complete blocks, at most `cap` of them.  Serial: one thread per frame.
+LZ_HD void frame_walk(const u8* p, u64 n, FrameInfoRec* fi, FrameBlockRec* blocks, u32 cap)
+{
+    fi->verdict = kFwOk; fi->tail = kTailTruncated; fi->skippable = 0; fi->ccksum = 0; fi->stored_cksum = 0;
+    fi->max_block = 0; fi->n_blocks = 0; fi->trunc_block = 0; fi->trunc_avail = 0; fi->content_size = 0;
+    if (n < 7) return;                                                      // frame.inl DS_storeHeader waits for 7 bytes
+    const u32 magic = rd_le32(p);
+    if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {
+        fi->skippable = 1;
+        if (n < 8) return;
+        const u64 sf = rd_le32(p + 4);
+        fi->tail = n - 8 < sf ? kTailTruncated : n - 8 > sf ? kTailTrailing : kTailSkippable;
+        return;
+    }
+    if (magic != 0x184D2206u) { fi->verdict = kFwFrameType; return; }
+    const u32 FLG = p[4];
+    const u32 fh = ((FLG >> 3) & 1) ? 15u : 7u;
+    if (n < fh) return;
+    const u32 BD = p[5], bsid = (BD >> 4) & 7;
+    if (((FLG >> 6) & 3) != 1) { fi->verdict = kFwHeaderVersion; return; }
+    if ((FLG >> 4) & 1) { fi->verdict = kFwBlockChecksum; return; }
+    if ((FLG & 3) || (BD & 0x80)) { fi->verdict = kFwReserved; return; }
+    if (bsid < 1) { fi->verdict = kFwMaxBlockSize; return; }
+    if (BD & 0x0F) { fi->verdict = kFwReserved; return; }
+    if ((u8)(xxh32_serial(p + 4, fh - 5, 0) >> 8) != p[fh - 1]) { fi->verdict = kFwHeaderChecksum; return; }
+    if (!((FLG >> 5) & 1)) { fi->verdict = kFwBlockMode; return; }             // linked blocks
+    fi->ccksum = (FLG >> 2) & 1;
+    fi->max_block = frame_block_bytes(bsid);
+    if (fh == 15) fi->content_size = rd_le64(p + 6);
+    u64 pos = fh;
+    u32 nb = 0;
+    for (;;) {
+        if (n - pos < 4) { fi->tail = kTailTruncated; break; }
+        const u32 word = rd_le32(p + pos);
+        const u32 csz = word & 0x7FFFFFFFu;
+        pos += 4;
+        if (csz == 0) {                                                     // end mark (the raw flag does not matter)
+            if (fi->ccksum) {
+                if (n - pos < 4) { fi->tail = kTailTruncated; break; }
+                fi->stored_cksum = rd_le32(p + pos);
+                pos += 4;
+            }
+            fi->tail = pos < n ? kTailTrailing : kTailEnd;
+            break;
+        }
+        if (csz > fi->max_block) { fi->tail = kTailGeneric; break; }
+        if (n - pos < csz) { fi->tail = kTailTruncated; fi->trunc_block = 1 + (word >> 31); fi->trunc_avail = n - pos; break; }
+        if (blocks && nb < cap) { blocks[nb].src = pos; blocks[nb].csize = csz; blocks[nb].raw = word >> 31; }
+        ++nb;
+        pos += csz;
+    }
+    fi->n_blocks = nb;
+}
+
+// Where a frame's decoded blocks go and what LizardF_decompress would say, block by block in frame order, given each
+// compressed block's Lizard_decompress_safe result at capacity max_block (`r`, ignored for raw blocks) and cap bytes of room.
+// Follows frame.inl's batch rule: a compressed block decoded straight into the output (room for a whole block at its
+// max-block-spaced slot of the current batch) fails with ERROR_GENERIC, one decoded through the context's one-block buffer
+// with ERROR_decompressionFailed.  The state lets the host settle a frame over several decode rounds.
+struct FrameSettle {
+    u64 dp;                // output bytes so far
+    u64 batch_at, batch_k; // the current in-place batch: where it started, slots taken after its first
+    u32 in_batch;
+    u32 verdict;           // kFwOk so far, or the frame's error
+    u32 open;              // 1 while blocks remain to be settled (verdict kFwOk)
+};
+LZ_HD void frame_settle_begin(const FrameInfoRec& fi, FrameSettle* st)
+{
+    st->dp = st->batch_at = st->batch_k = 0; st->in_batch = 0; st->verdict = fi.verdict; st->open = 0;
+    if (fi.verdict != kFwOk) return;
+    if (fi.skippable) { st->verdict = fi.tail == kTailSkippable ? kFwOk : kFwFrameSize; return; }
+    st->open = 1;
+}
+// the next block: returns its offset in the output; on an error closes the frame with that verdict
+LZ_HD u64 frame_settle_block(const FrameInfoRec& fi, const FrameBlockRec& b, int r, u64 cap, FrameSettle* st)
+{
+    const u64 mb = fi.max_block, at = st->dp;
+    u32 v = kFwOk;
+    if (b.raw) {
+        st->in_batch = 0;
+        if (b.csize > cap - at) v = kFwDstTooSmall;
+        else st->dp += b.csize;
+    } else {
+        const u64 slot = st->batch_at + (st->batch_k + 1) * mb;
+        if (st->in_batch && slot <= cap && cap - slot >= mb) {              // next slot of the same batch
+            ++st->batch_k;
+            if (r < 0) v = kFwGeneric; else st->dp += (u64)r;
+        } else {
+            st->in_batch = 0;
+            const u64 room = cap - at;
+            if (room == 0) v = kFwDstTooSmall;
+            else if (room >= mb) {                                          // a new batch, decoded in place
+                st->in_batch = 1; st->batch_at = at; st->batch_k = 0;
+                if (r < 0) v = kFwGeneric; else st->dp += (u64)r;
+            }
+            else if (r < 0) v = kFwDecompressionFailed;                     // through the one-block buffer
+            else if ((u64)r > room) v = kFwDstTooSmall;
+            else st->dp += (u64)r;
+        }
+    }
+    if (v != kFwOk) { st->verdict = v; st->open = 0; }
+    return at;
+}
+// after the frame's last complete block: the verdict of its tail; *check_hash = 1 when the verdict still depends on the
+// content checksum over the placed output (frame_settle_hash)
+LZ_HD u32 frame_settle_end(const FrameInfoRec& fi, u64 cap, FrameSettle* st, u32* check_hash)
+{
+    *check_hash = 0;
+    st->open = 0;
+    const u64 dp = st->dp;
+    u32 v = kFwOk;
+    if (fi.tail == kTailGeneric) v = kFwGeneric;
+    else if (fi.tail == kTailTruncated) {
+        // LizardF_decompress stops in a truncated block with input left over when the output is full first: a raw block
+        // copies what fits, a compressed one is not started when no room is left
+        const u64 room = cap - dp;
+        v = (fi.trunc_block == 2 ? fi.trunc_avail > room : fi.trunc_block == 1 && room == 0 && fi.trunc_avail > 0) ? kFwDstTooSmall
+                                                                                                               : kFwFrameSize;
+    }
+    else if (fi.content_size && fi.content_size != dp) v = kFwFrameSize;
+    else if (fi.ccksum) *check_hash = 1;
+    else if (fi.tail == kTailTrailing) v = kFwFrameSize;
+    st->verdict = v;
+    return v;
+}
+// the whole frame at once (the host shim): place[k] for every block, *out = total size
+LZ_HD u32 frame_settle(const FrameInfoRec& fi, const FrameBlockRec* blocks, const int* decoded, u64 cap, u64* place,
+                       u64* out, u32* check_hash)
+{
+    FrameSettle st;
+    frame_settle_begin(fi, &st);
+    *out = 0; *check_hash = 0;
+    for (u32 k = 0; st.open && k < fi.n_blocks; ++k) place[k] = frame_settle_block(fi, blocks[k], decoded[k], cap, &st);
+    if (!st.open) return st.verdict;
+    *out = st.dp;
+    return frame_settle_end(fi, cap, &st, check_hash);
+}
+// the verdict once the content checksum is known (frame_settle gave kFwOk with check_hash)
+LZ_HD u32 frame_settle_hash(const FrameInfoRec& fi, u32 hash)
+{
+    if (hash != fi.stored_cksum) return kFwContentChecksum;
+    return fi.tail == kTailTrailing ? kFwFrameSize : kFwOk;
+}
+
+}  // namespace lzb

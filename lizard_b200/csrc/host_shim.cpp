@@ -17,6 +17,7 @@
 #include "encode_opt.cuh"
 #include "decode.cuh"
 #include "decode2.cuh"
+#include "frame_device.cuh"
 #include <stdlib.h>
 
 extern "C" int lzb_host_huf_decompress(unsigned char* dst, unsigned n, const unsigned char* src, unsigned c)
@@ -813,4 +814,42 @@ extern "C" int lzb_dict_compress(const unsigned char* src, int n, unsigned char*
     else dict_compress_body<lzb::HostLanes>(&a);
     free(a.work->huf.seg_count); free(a.work); free(a.dchain); free(a.sh); free(a.ov);
     return a.result;
+}
+
+// XXH32 as the frame kernels compute it (frame_device.cuh), one thread
+extern "C" unsigned lzb_host_xxh32(const unsigned char* p, unsigned long long n, unsigned seed) { return lzb::xxh32_serial(p, n, seed); }
+
+// LizardB200_decompressFrames for one frame on the host: the index kernel's walk, each compressed block through the one-lane
+// decoder at the frame's maximum block size, frame_settle, placement and the checksum.  Returns the result as a size_t
+// (LizardF error codes are negated); `blocks_out` = number of complete blocks the walk found.
+extern "C" unsigned long long lzb_host_frame_decode(const unsigned char* src, unsigned long long n, unsigned char* dst,
+                                                    unsigned long long cap, unsigned* blocks_out)
+{
+    lzb::FrameInfoRec fi;
+    lzb::frame_walk(src, n, &fi, nullptr, 0);
+    if (blocks_out) *blocks_out = fi.n_blocks;
+    const unsigned nb = fi.verdict == lzb::kFwOk && !fi.skippable ? fi.n_blocks : 0;
+    lzb::FrameBlockRec* blocks = (lzb::FrameBlockRec*)malloc((nb + 1) * sizeof(lzb::FrameBlockRec));
+    int* decoded = (int*)calloc(nb + 1, sizeof(int));
+    lzb::u64* place = (lzb::u64*)malloc((nb + 1) * 8);
+    unsigned char** staged = (unsigned char**)calloc(nb + 1, sizeof(unsigned char*));
+    if (nb) lzb::frame_walk(src, n, &fi, blocks, nb);
+    for (unsigned k = 0; k < nb; ++k) {
+        if (blocks[k].raw) continue;
+        staged[k] = (unsigned char*)malloc(fi.max_block + 64);
+        decoded[k] = lzb_host_decompress(src + blocks[k].src, (int)blocks[k].csize, staged[k], (int)fi.max_block);
+    }
+    lzb::u64 out = 0; lzb::u32 check = 0;
+    lzb::u32 v = lzb::frame_settle(fi, blocks, decoded, cap, place, &out, &check);
+    if (v == lzb::kFwOk && !fi.skippable) {
+        for (unsigned k = 0; k < nb; ++k) {
+            if (blocks[k].raw) memcpy(dst + place[k], src + blocks[k].src, blocks[k].csize);
+            else if (decoded[k] > 0) memcpy(dst + place[k], staged[k], (size_t)decoded[k]);
+        }
+        if (check) v = lzb::frame_settle_hash(fi, lzb::xxh32_serial(dst, out, 0));
+    }
+    for (unsigned k = 0; k < nb; ++k) free(staged[k]);
+    free(staged); free(place); free(decoded); free(blocks);
+    if (v != lzb::kFwOk) return (unsigned long long)-(long long)v;
+    return fi.skippable ? 0 : out;
 }
