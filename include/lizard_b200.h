@@ -240,7 +240,10 @@ int LizardB200_decompress_blocks(const void* src, size_t srcStride, const int* c
  * (growing it -- the first call, or a batch larger than any before -- is the one case in which these calls synchronise the
  * stream and allocate; do not capture that call in a CUDA graph).  Calls on DIFFERENT streams are serialised against each
  * other on the device (each launch waits for the previous launch's completion event when the stream changes), so results
- * do not depend on how the caller spreads calls over streams; calls on one stream run in stream order. */
+ * do not depend on how the caller spreads calls over streams; calls on one stream run in stream order.  The exception: a call
+ * made while its stream is being captured into a CUDA graph neither waits for nor records that event (an event recorded
+ * outside a capture cannot be waited on inside it), so the graph's launches are not serialised against the library's other
+ * calls; the caller orders graph launches against them. */
 int LizardB200_decompress_device(const void* dSrc, const uint64_t* dSrcOff, const uint32_t* dSrcLen,
                                  void* dDst, const uint64_t* dDstOff, const uint32_t* dDstCap,
                                  int* dResult, unsigned nUnits, void* cudaStream);
@@ -306,6 +309,30 @@ int LizardB200_compressFrames(const void* dSrc, const uint64_t* srcOff, const ui
 int LizardB200_decompressFrames(const void* dSrc, const uint64_t* srcOff, const uint64_t* srcSize,
                                 void* dDst, const uint64_t* dstOff, const uint64_t* dstCap,
                                 size_t* result, unsigned nFrames, void* cudaStream);
+/* LizardB200_decompressFrames with EVERYTHING in device memory -- payload, the offset, size and capacity tables and the results
+ * dResult[i] (a size_t that LizardF_isError tests) -- and enqueue-only (DESIGN.md 3.4b).  nFrames, maxBlocks and stageBytes are
+ * host values; they fix the grids and the workspace.  Frames are admitted in index order, as a prefix: frame i is admitted while
+ * the complete blocks of frames 0..i number at most maxBlocks and their compressed blocks' staging slots (the frame's maximum
+ * block size each) take at most stageBytes.  A frame whose header check fails, a skippable frame and an empty one take
+ * nothing.  An admitted frame gets exactly what LizardB200_decompressFrames gives it, in result and bytes; a frame that is not
+ * admitted gets LizardF_ERROR_allocation_failed and nothing is written to its range.  There is one decode round: the caller
+ * chooses the bounds.
+ * Stream and capture rules.  The workspace (tables for nFrames and maxBlocks, stageBytes of slots) is library-owned and grows on
+ * demand; the growing call synchronises `cudaStream` and allocates.  A call that needs no growth issues no host<->device copy,
+ * no synchronisation and no allocation: it enqueues a sequence of launches that depends only on (nFrames, maxBlocks,
+ * stageBytes, decode variant), so after one call of the same or a larger shape it can be captured in a CUDA graph, and each
+ * replay decodes whatever frames the tables then point at.  A captured call neither waits for nor signals the other streams'
+ * use of the shared workspace (the exception above): order the graph's launches against the library's other calls on the
+ * device yourself, and capture again after any call grows the workspace (a larger shape, or another device call with a larger
+ * batch).  A capture that would have to grow the workspace -- the frame tables, the staging arena or the decoder's pre-pass
+ * workspaces -- returns LIZARDB200_ERR_ARGUMENT and enqueues nothing.  stageBytes above maxBlocks slots of the largest maximum
+ * block size (256 MiB) admits the same frames as that bound, and the arena is never sized above it, so SIZE_MAX means "no
+ * staging bound".  LIZARDB200_ERR_ARGUMENT also for null tables when nFrames > 0; LIZARDB200_ERR_MEMORY when the workspace
+ * cannot grow. */
+int LizardB200_decompressFramesAsync(const void* dSrc, const uint64_t* dSrcOff, const uint64_t* dSrcSize,
+                                     void* dDst, const uint64_t* dDstOff, const uint64_t* dDstCap,
+                                     size_t* dResult, unsigned nFrames,
+                                     unsigned maxBlocks, size_t stageBytes, void* cudaStream);
 /* diagnostics: launch shape of the encode kernel for a level (no device needed): warps per CTA, how many of them keep their
  * hash table in shared memory, CTAs per SM (an upper bound: a launch holds no more than fit), dynamic shared memory per CTA.
  * The level's default, or LIZARDB200_ENC_SHAPE="warps,tables,ctas" when that is set and valid, exactly as the encoder

@@ -9,6 +9,7 @@
 #include "encode_opt_kernel.cuh"
 #include "encode_dict_kernel.cuh"
 #include "frame_device_kernels.cuh"
+#include "frame_async_kernels.cuh"
 
 #include <cuda_runtime.h>
 #include <mutex>
@@ -232,6 +233,7 @@ struct Context {
     DeviceBuffer d_progress;
     DeviceBuffer d_in, d_out, d_tab, d_pack;
     DeviceBuffer fd_tab, fd_stage;            // tables and staged blocks of the device-memory frame calls (frame.inl)
+    DeviceBuffer fa_tab, fa_stage;            // the same for LizardB200_decompressFramesAsync, kept apart: a captured graph holds them
     EncodeConfig enc_cfg;
 };
 Context g_ctx[kMaxDevices];
@@ -363,13 +365,21 @@ int ensure_context(Context& c, int device)
 }
 
 // workspace hand-over between streams (see Context::ws_done)
+// A stream being captured into a CUDA graph neither waits for nor records the hand-over event: an event recorded outside the
+// capture cannot be waited on inside it, and the graph's launches are ordered by whoever launches the graph.
+bool stream_capturing(cudaStream_t s)
+{
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    return cudaStreamIsCapturing(s, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone;
+}
 void workspace_acquire(Context& c, cudaStream_t s)
 {
     if (!c.ws_done) cudaEventCreateWithFlags(&c.ws_done, cudaEventDisableTiming);
-    if (c.ws_used && c.ws_stream != s && c.ws_done) cudaStreamWaitEvent(s, c.ws_done, 0);
+    if (c.ws_used && c.ws_stream != s && c.ws_done && !stream_capturing(s)) cudaStreamWaitEvent(s, c.ws_done, 0);
 }
 void workspace_release(Context& c, cudaStream_t s)
 {
+    if (stream_capturing(s)) return;
     if (c.ws_done) cudaEventRecord(c.ws_done, s);
     c.ws_stream = s; c.ws_used = true;
 }
@@ -392,13 +402,20 @@ constexpr size_t kPrepassArenaMax = (size_t)3 << 30;    // never more than this,
                                                         // rest to the in-kernel expansion (a batch of a million 4 KiB units must
                                                         // not ask for 160 KiB each)
 
+// the pre-pass workspaces a batch of n units needs
+void prepass_bytes(const Context& c, size_t n, size_t* ws_bytes, size_t* arena_bytes, size_t* scratch_bytes)
+{
+    *ws_bytes = 256 + n * sizeof(UnitPre) + 2 * n * sizeof(HufJob);
+    *arena_bytes = n * kPrepassArenaPerUnit;
+    if (*arena_bytes > kPrepassArenaMax) *arena_bytes = kPrepassArenaMax;
+    *scratch_bytes = (size_t)c.sm_count * c.exp_ctas * kExpWarps * kExpJobs * sizeof(HufJobScratch);
+}
+
 int launch_prepass(Context& c, DecodeBatch& b, cudaStream_t s)
 {
     const size_t n = b.n_units;
-    const size_t ws_bytes = 256 + n * sizeof(UnitPre) + 2 * n * sizeof(HufJob);
-    size_t arena_bytes = n * kPrepassArenaPerUnit;
-    if (arena_bytes > kPrepassArenaMax) arena_bytes = kPrepassArenaMax;
-    const size_t scratch_bytes = (size_t)c.sm_count * c.exp_ctas * kExpWarps * kExpJobs * sizeof(HufJobScratch);
+    size_t ws_bytes, arena_bytes, scratch_bytes;
+    prepass_bytes(c, n, &ws_bytes, &arena_bytes, &scratch_bytes);
     if (ws_bytes > c.pre_ws.bytes || arena_bytes > c.pre_arena.bytes || scratch_bytes > c.pre_scratch.bytes) {
         // growing a workspace is the one place where an enqueue-only call synchronises (first call, or a larger batch than
         // ever before): an earlier launch may still be reading the buffers that are about to be replaced
@@ -430,12 +447,19 @@ int launch_prepass(Context& c, DecodeBatch& b, cudaStream_t s)
 // records; runs behind the Huffman pre-pass (it reads the expanded streams) and ahead of the token kernel.
 constexpr size_t kSeqRecordsPerUnit = 2048;             // 32 KiB of records per unit on average; overflow falls back in-kernel
 
+// the token pre-pass workspaces a batch of n units needs
+void token_parse_bytes(size_t n, size_t* ws_bytes, size_t* rec_bytes)
+{
+    *ws_bytes = 64 + n * sizeof(UnitSeq);
+    *rec_bytes = n * kSeqRecordsPerUnit * sizeof(PoolRun);
+    if (*rec_bytes < ((size_t)64 << 20)) *rec_bytes = (size_t)64 << 20;
+}
+
 int launch_token_parse(Context& c, DecodeBatch& b, cudaStream_t s)
 {
     const size_t n = b.n_units;
-    const size_t ws_bytes = 64 + n * sizeof(UnitSeq);
-    size_t rec_bytes = n * kSeqRecordsPerUnit * sizeof(PoolRun);
-    if (rec_bytes < ((size_t)64 << 20)) rec_bytes = (size_t)64 << 20;
+    size_t ws_bytes, rec_bytes;
+    token_parse_bytes(n, &ws_bytes, &rec_bytes);
     if (ws_bytes > c.seq_ws.bytes || rec_bytes > c.seq_recs.bytes) {
         cudaStreamSynchronize(s);
         if (c.seq_ws.reserve(ws_bytes) != cudaSuccess || c.seq_recs.reserve(rec_bytes) != cudaSuccess) {
@@ -456,6 +480,23 @@ int launch_token_parse(Context& c, DecodeBatch& b, cudaStream_t s)
     CU_OK(cudaGetLastError());
     b.seq = q.seq; b.recs = q.recs;
     return LIZARDB200_OK;
+}
+
+// true when launch_decode of n units (no progress) finds every pre-pass workspace it will use large enough, so that it
+// neither synchronises nor allocates (the condition for capturing it in a CUDA graph)
+bool decode_workspace_fits(const Context& c, u32 n)
+{
+    if ((c.dec_variant & 4) && n >= kPrepassMinUnits) {
+        size_t ws, arena, scratch;
+        prepass_bytes(c, n, &ws, &arena, &scratch);
+        if (ws > c.pre_ws.bytes || arena > c.pre_arena.bytes || scratch > c.pre_scratch.bytes) return false;
+    }
+    if ((c.dec_variant & 8) && !(c.dec_variant & 16) && n >= kPrepassMinUnits) {
+        size_t ws, recs;
+        token_parse_bytes(n, &ws, &recs);
+        if (ws > c.seq_ws.bytes || recs > c.seq_recs.bytes) return false;
+    }
+    return true;
 }
 
 int launch_decode(Context& c, const void* dSrc, const u64* dSrcOff, const u32* dSrcLen,

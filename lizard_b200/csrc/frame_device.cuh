@@ -219,4 +219,64 @@ LZ_HD u32 frame_settle_hash(const FrameInfoRec& fi, u32 hash)
     return fi.tail == kTailTrailing ? kFwFrameSize : kFwOk;
 }
 
+// ---- LizardB200_decompressFramesAsync (DESIGN.md 3.4b): admission and settling on the device-side layout -------------------
+// Admission is a prefix over frames in index order.  Frame i is admitted while the inclusive sum of the blocks taken by frames
+// 0..i stays within max_blocks and the inclusive sum of their slot bytes (one slot of the frame's maximum block size per
+// compressed block) within stage_bytes.  A frame whose header fails, a skippable frame and an empty frame take nothing.  The
+// kernels apply the two bounds one after the other (the slot bytes are only known once the admitted frames' blocks are
+// indexed); both sums grow with i, so the two steps admit the same prefix as the rule above.
+constexpr u32 kFwAllocation = 9;                                            // LizardF_ERROR_allocation_failed
+LZ_HD u64 frame_plan_blocks(const FrameInfoRec& fi) { return fi.verdict == kFwOk && !fi.skippable ? fi.n_blocks : 0; }
+LZ_HD u64 frame_plan_slots(const FrameInfoRec& fi, const FrameBlockRec* blocks)
+{
+    u64 s = 0;
+    const u32 nb = (u32)frame_plan_blocks(fi);
+    for (u32 k = 0; k < nb; ++k) s += blocks[k].raw ? 0 : fi.max_block;
+    return s;
+}
+// step 1: blocks before the frame (exclusive sum) and its own; step 2: slot bytes likewise, for a frame that passed step 1
+LZ_HD bool frame_admit_blocks(u64 before, u64 blocks, u32 max_blocks) { return before + blocks <= max_blocks; }
+LZ_HD bool frame_admit_slots(u64 before, u64 slots, u64 stage_bytes) { return before + slots <= stage_bytes; }
+// The staging bytes a call can ever use: max_blocks slots of the largest maximum block size (256 MiB).  A larger stageBytes,
+// up to SIZE_MAX for "no bound", admits the same frames, so the call sizes its arena by this and never by more.
+LZ_HD u64 frame_stage_limit(u32 max_blocks, u64 stage_bytes)
+{
+    const u64 most = (u64)max_blocks * frame_block_bytes(7);
+    return stage_bytes < most ? stage_bytes : most;
+}
+
+// Per-block gather entries of one frame: staged (decoded bytes from the staging arena) and raw (stored bytes from the
+// frame).  Length 0 where a block is not placed.
+struct FrameGather {
+    u64* s_off; u64* s_dst; int* s_len;
+    u64* r_off; u64* r_dst; int* r_len;
+};
+// frame_settle over one admitted frame laid out as the device keeps it: blocks[k], the block's decode result res[k] and its
+// staging slot stage[k] (both ignored for raw blocks).  Writes one staged and one raw entry per block, the frame's source at
+// src_at and its output at dst_at; returns the verdict before the content checksum (frame_settle).
+LZ_HD u32 frame_settle_entries(const FrameInfoRec& fi, const FrameBlockRec* blocks, const int* res, const u64* stage,
+                               u64 src_at, u64 dst_at, u64 cap, const FrameGather& g, u64* out, u32* check_hash)
+{
+    FrameSettle st;
+    frame_settle_begin(fi, &st);
+    *out = 0; *check_hash = 0;
+    const u32 nb = (u32)frame_plan_blocks(fi);
+    for (u32 k = 0; k < nb; ++k) {
+        const FrameBlockRec b = blocks[k];
+        int sl = 0, rl = 0;
+        u64 d = dst_at;
+        if (st.open) {
+            const int r = b.raw ? 0 : res[k];
+            d += frame_settle_block(fi, b, r, cap, &st);
+            if (st.open && b.raw) rl = (int)b.csize;
+            else if (st.open && r > 0) sl = r;
+        }
+        g.s_off[k] = b.raw ? 0 : stage[k]; g.s_dst[k] = d; g.s_len[k] = sl;
+        g.r_off[k] = src_at + b.src;        g.r_dst[k] = d; g.r_len[k] = rl;
+    }
+    if (!st.open) return st.verdict;
+    *out = st.dp;
+    return frame_settle_end(fi, cap, &st, check_hash);
+}
+
 }  // namespace lzb

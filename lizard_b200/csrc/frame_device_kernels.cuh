@@ -24,10 +24,10 @@ __global__ void __launch_bounds__(128) lizard_frame_index_kernel(const u8* src, 
 // the four accumulators over the piece's stripes, and lane 0 merges them and hashes the tail.  The recurrence stays serial:
 // one buffer hashes at one warp's rate.  Buffer f's hash goes to out[slot[f]] (slot null: out[f]).
 constexpr u32 kHashWarps = 4, kHashPiece = 4096, kHashWords = kHashPiece / 16 + 1;
-__global__ void __launch_bounds__(kHashWarps * 32) lizard_frame_hash_kernel(const u8* base, const u64* off, const u64* len, u32 n,
-                                                                           u32* out, const u32* slot)
+// the loop of both hash kernels (n: the number of buffers, read by the caller)
+__device__ __forceinline__ void frame_hash_buffers(uint4 (*stage)[kHashWords + 1], const u8* base, const u64* off, const u64* len,
+                                                   u32 n, u32* out, const u32* slot)
 {
-    __shared__ __align__(16) uint4 stage[kHashWarps][kHashWords + 1];
     const u32 warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     constexpr u32 kPer = (kHashWords + 31) / 32;
     for (u32 f = blockIdx.x * kHashWarps + warp; f < n; f += gridDim.x * kHashWarps) {
@@ -77,6 +77,12 @@ __global__ void __launch_bounds__(kHashWarps * 32) lizard_frame_hash_kernel(cons
         if (!pieces && lane == 0) { const u32 z[4] = { 0, 0, 0, 0 }; out[slot ? slot[f] : f] = xx_finish(z, 0, nullptr, 0, 0); }
         __syncwarp();
     }
+}
+__global__ void __launch_bounds__(kHashWarps * 32) lizard_frame_hash_kernel(const u8* base, const u64* off, const u64* len, u32 n,
+                                                                           u32* out, const u32* slot)
+{
+    __shared__ __align__(16) uint4 stage[kHashWarps][kHashWords + 1];
+    frame_hash_buffers(stage, base, off, len, n, out, slot);
 }
 
 // Frame assembly, compressing.  Block k of the call belongs to frame frame_of[k]; blocks of one frame are consecutive,

@@ -6,6 +6,7 @@
 #include <stddef.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <vector>
 #define LZB_SHIM_CHECK(cond) do { if (!(cond)) { fprintf(stderr, "host shim check failed: %s (%s:%d)\n", #cond, __FILE__, __LINE__); abort(); } } while (0)
 #define LZB_DICT_STATS 1          /* count the dictionary decoder's matches (lzb_dict_stats) */
 #define LZB_LP_STATS 1            /* count the lowestPrice parser's rare paths (lzb_lp_stats) */
@@ -850,6 +851,76 @@ extern "C" unsigned long long lzb_host_frame_decode(const unsigned char* src, un
     }
     for (unsigned k = 0; k < nb; ++k) free(staged[k]);
     free(staged); free(place); free(decoded); free(blocks);
+    if (v != lzb::kFwOk) return (unsigned long long)-(long long)v;
+    return fi.skippable ? 0 : out;
+}
+
+// the staging arena LizardB200_decompressFramesAsync sizes for (max_blocks, stage_bytes)
+extern "C" unsigned long long lzb_host_frame_stage_limit(unsigned max_blocks, unsigned long long stage_bytes)
+{
+    return lzb::frame_stage_limit(max_blocks, stage_bytes);
+}
+
+// LizardB200_decompressFramesAsync's planning (frame_async_kernels.cuh) serially: frame i takes blocks[i] blocks and, if it
+// passes the block bound, slots[i] bytes of slots; ok[i] = 0 marks a frame whose header check failed.  Writes adm[i] and, for
+// admitted frames, the block base and slot base the kernels give them.
+// The stage bound is clamped first, as LizardB200_decompressFramesAsync clamps it (frame_stage_limit).
+extern "C" void lzb_host_frame_async_plan(unsigned n, const unsigned long long* blocks, const unsigned long long* slots,
+                                          const unsigned* ok, unsigned max_blocks, unsigned long long stage_bytes,
+                                          unsigned* adm, unsigned long long* base, unsigned long long* slot)
+{
+    stage_bytes = lzb::frame_stage_limit(max_blocks, stage_bytes);
+    std::vector<lzb::FrameInfoRec> fi(n);
+    for (unsigned i = 0; i < n; ++i) {
+        memset(&fi[i], 0, sizeof fi[i]);
+        fi[i].verdict = ok[i] ? lzb::kFwOk : lzb::kFwFrameType;
+        fi[i].n_blocks = (lzb::u32)blocks[i];
+    }
+    lzb::u64 before = 0;
+    for (unsigned i = 0; i < n; ++i) {                                       // step 1: blocks
+        const lzb::u64 v = lzb::frame_plan_blocks(fi[i]);
+        adm[i] = lzb::frame_admit_blocks(before, v, max_blocks);
+        base[i] = before;
+        before += v;
+    }
+    before = 0;
+    for (unsigned i = 0; i < n; ++i) {                                       // step 2: slots of the frames that passed step 1
+        const lzb::u64 v = adm[i] && lzb::frame_plan_blocks(fi[i]) ? slots[i] : 0;     // as frame_plan_slots
+        adm[i] = adm[i] && lzb::frame_admit_slots(before, v, stage_bytes);
+        slot[i] = before;
+        before += v;
+    }
+}
+
+// One frame through LizardB200_decompressFramesAsync's layout: the walk, blocks decoded by the one-lane decoder into slots
+// of the maximum block size behind each other in one staging arena, frame_settle_entries, the moves its gather entries
+// describe (staged, then raw), the checksum.  Same return convention as lzb_host_frame_decode.
+extern "C" unsigned long long lzb_host_frame_async_decode(const unsigned char* src, unsigned long long n, unsigned char* dst,
+                                                          unsigned long long cap)
+{
+    lzb::FrameInfoRec fi;
+    lzb::frame_walk(src, n, &fi, nullptr, 0);
+    const unsigned nb = (unsigned)lzb::frame_plan_blocks(fi);
+    std::vector<lzb::FrameBlockRec> blocks(nb + 1);
+    if (nb) lzb::frame_walk(src, n, &fi, blocks.data(), nb);
+    const lzb::u64 slots = lzb::frame_plan_slots(fi, blocks.data());
+    std::vector<unsigned char> stage(slots + 64);
+    std::vector<int> res(nb + 1, 0);
+    std::vector<lzb::u64> at(nb + 1, 0), s_off(nb + 1), s_dst(nb + 1), r_off(nb + 1), r_dst(nb + 1);
+    std::vector<int> s_len(nb + 1), r_len(nb + 1);
+    lzb::u64 slot = 0;
+    for (unsigned k = 0; k < nb; ++k) {
+        if (blocks[k].raw) continue;
+        at[k] = slot;
+        res[k] = lzb_host_decompress(src + blocks[k].src, (int)blocks[k].csize, stage.data() + slot, (int)fi.max_block);
+        slot += fi.max_block;
+    }
+    const lzb::FrameGather g{ s_off.data(), s_dst.data(), s_len.data(), r_off.data(), r_dst.data(), r_len.data() };
+    lzb::u64 out = 0; lzb::u32 check = 0;
+    lzb::u32 v = lzb::frame_settle_entries(fi, blocks.data(), res.data(), at.data(), 0, 0, cap, g, &out, &check);
+    for (unsigned k = 0; k < nb; ++k) if (s_len[k] > 0) memcpy(dst + s_dst[k], stage.data() + s_off[k], (size_t)s_len[k]);
+    for (unsigned k = 0; k < nb; ++k) if (r_len[k] > 0) memcpy(dst + r_dst[k], src + r_off[k], (size_t)r_len[k]);
+    if (check) v = lzb::frame_settle_hash(fi, lzb::xxh32_serial(dst, out, 0));
     if (v != lzb::kFwOk) return (unsigned long long)-(long long)v;
     return fi.skippable ? 0 : out;
 }
