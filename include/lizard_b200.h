@@ -333,6 +333,27 @@ int LizardB200_decompressFramesAsync(const void* dSrc, const uint64_t* dSrcOff, 
                                      void* dDst, const uint64_t* dDstOff, const uint64_t* dDstCap,
                                      size_t* dResult, unsigned nFrames,
                                      unsigned maxBlocks, size_t stageBytes, void* cudaStream);
+/* LizardB200_compressFrames with the offset, size and capacity tables and the results dResult[i] in device memory, and
+ * enqueue-only (DESIGN.md 3.4c).  prefs is a host pointer: one set of preferences for the whole call (NULL: zeroed).  nFrames,
+ * maxBlocks, stageBytes and prefs are host values; they fix the grids, the workspace and the launch sequence.  Frames are
+ * admitted in index order, as a prefix: frame i is admitted while the blocks of frames 0..i number at most maxBlocks and their
+ * staging bytes (each block's input length rounded up to 16) stay within stageBytes.  A frame that fails
+ * LizardF_compressFrame's checks (bound, block size ID, block mode, level) and an empty frame take nothing.  An admitted frame
+ * gets exactly what LizardB200_compressFrames gives it, in result and bytes (the 1-byte content-size case above included); a
+ * frame that is not admitted gets LizardF_ERROR_allocation_failed and nothing is written to its range.  stageBytes above
+ * maxBlocks blocks of the preferences' block size (256 MiB for an invalid block size ID) admits the same frames as that bound,
+ * and the arena is never sized above it, so SIZE_MAX means "no staging bound".
+ * Stream and capture rules as for LizardB200_decompressFramesAsync: the workspace (tables for nFrames and maxBlocks, stageBytes
+ * of encoded blocks) grows on demand and the growing call synchronises `cudaStream`; a call that needs no growth issues no
+ * host<->device copy, no synchronisation and no allocation, and can be captured in a CUDA graph after one call of the same or a
+ * larger shape; each replay compresses whatever the tables then point at.  A capture that would have to grow the workspace
+ * returns LIZARDB200_ERR_ARGUMENT and enqueues nothing.  Its workspace is its own: no other call of the library moves it.
+ * LIZARDB200_ERR_ARGUMENT also for null tables when nFrames > 0; LIZARDB200_ERR_MEMORY when the workspace cannot grow.
+ * The encoder's grid holds every SM while it runs: the call does not overlap other kernels during the encode. */
+int LizardB200_compressFramesAsync(const void* dSrc, const uint64_t* dSrcOff, const uint64_t* dSrcSize,
+                                   void* dDst, const uint64_t* dDstOff, const uint64_t* dDstCap,
+                                   size_t* dResult, unsigned nFrames, const LizardF_preferences_t* prefs,
+                                   unsigned maxBlocks, size_t stageBytes, void* cudaStream);
 /* diagnostics: launch shape of the encode kernel for a level (no device needed): warps per CTA, how many of them keep their
  * hash table in shared memory, CTAs per SM (an upper bound: a launch holds no more than fit), dynamic shared memory per CTA.
  * The level's default, or LIZARDB200_ENC_SHAPE="warps,tables,ctas" when that is set and valid, exactly as the encoder

@@ -76,6 +76,8 @@ def lib():
                                                   ctypes.POINTER(ctypes.c_size_t), ctypes.c_uint, ctypes.c_void_p]
         L.LizardB200_decompressFramesAsync.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_uint, ctypes.c_uint, ctypes.c_size_t,
                                                                                ctypes.c_void_p]
+        L.LizardB200_compressFramesAsync.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_uint, ctypes.c_void_p, ctypes.c_uint,
+                                                     ctypes.c_size_t, ctypes.c_void_p]
         L.LizardF_isError.argtypes = [ctypes.c_size_t]
         L.LizardF_getErrorName.argtypes = [ctypes.c_size_t]
         L.LizardF_getErrorName.restype = ctypes.c_char_p
@@ -388,29 +390,23 @@ def decompress_frames(d_src: int, src_off, src_size, d_dst: int, dst_off, dst_ca
     return list(res)
 
 
-def decompress_frames_async(d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_cap, d_result, max_blocks: int,
-                            stage_bytes: int, stream=None, n_frames: int = None):
-    """LizardB200_decompressFramesAsync: decompress_frames with the tables and the results in device memory, enqueue-only and
-    capturable in a CUDA graph after one call of the same shape (include/lizard_b200.h).  Frames are admitted in index order
-    while their blocks number at most max_blocks and their staging slots take at most stage_bytes; the others get
-    ERROR_allocation_failed.  Every argument is a device address as an integer or a CUDA tensor (the tables 8-byte integers,
-    one per frame; d_result 8 bytes per frame).  n_frames defaults to the length of a tensor table; `stream` to the current
-    torch stream when tensors are given, else 0 (the default stream).  Returns nothing: read d_result after the stream's work."""
-    args = [d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_cap, d_result]
+def _async_frame_args(args, n_frames, stream):
+    """The device addresses, n_frames and stream of a device-table frame call: args are the source, its offset and size tables,
+    the destination, its offset and capacity tables and the results, each a device address as an integer or a CUDA tensor."""
     tensors = [a for a in args if not isinstance(a, int)]
     for a in tensors:
         if not (a.is_cuda and a.is_contiguous()):
             raise ValueError("tensor arguments must be contiguous CUDA tensors")
-    for a in args[1:3] + args[4:]:
-        if not isinstance(a, int) and a.element_size() != 8:
+    tables = [a for a in args[1:3] + args[4:] if not isinstance(a, int)]
+    for a in tables:
+        if a.element_size() != 8:
             raise ValueError("the offset, size and capacity tables and the results hold 8-byte integers")
     if n_frames is None:
-        sized = [a for a in args[1:3] + args[4:] if not isinstance(a, int)]
-        if not sized:
+        if not tables:
             raise ValueError("n_frames is needed when every table is an address")
-        n_frames = sized[0].numel()
-    for a in args[1:3] + args[4:]:
-        if not isinstance(a, int) and a.numel() < n_frames:
+        n_frames = tables[0].numel()
+    for a in tables:
+        if a.numel() < n_frames:
             raise ValueError("a table holds fewer entries than n_frames")
     if stream is None:
         if tensors:
@@ -420,9 +416,35 @@ def decompress_frames_async(d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_ds
             stream = 0
     elif not isinstance(stream, int):
         stream = stream.cuda_stream
-    ptr = [a if isinstance(a, int) else a.data_ptr() for a in args]
+    return [a if isinstance(a, int) else a.data_ptr() for a in args], n_frames, stream
+
+
+def decompress_frames_async(d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_cap, d_result, max_blocks: int,
+                            stage_bytes: int, stream=None, n_frames: int = None):
+    """LizardB200_decompressFramesAsync: decompress_frames with the tables and the results in device memory, enqueue-only and
+    capturable in a CUDA graph after one call of the same shape (include/lizard_b200.h).  Frames are admitted in index order
+    while their blocks number at most max_blocks and their staging slots take at most stage_bytes; the others get
+    ERROR_allocation_failed.  Every argument is a device address as an integer or a CUDA tensor (the tables 8-byte integers,
+    one per frame; d_result 8 bytes per frame).  n_frames defaults to the length of a tensor table; `stream` to the current
+    torch stream when tensors are given, else 0 (the default stream).  Returns nothing: read d_result after the stream's work."""
+    ptr, n_frames, stream = _async_frame_args([d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_cap, d_result], n_frames,
+                                              stream)
     _check(lib().LizardB200_decompressFramesAsync(*ptr, n_frames, max_blocks, stage_bytes, stream or None),
            "LizardB200_decompressFramesAsync")
+
+
+def compress_frames_async(d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_cap, d_result, prefs, max_blocks: int,
+                          stage_bytes: int, stream=None, n_frames: int = None):
+    """LizardB200_compressFramesAsync: compress_frames with the tables and the results in device memory, enqueue-only and
+    capturable in a CUDA graph after one call of the same shape (include/lizard_b200.h).  `prefs` is one Preferences for every
+    frame (make_prefs; None = zeroed).  Frames are admitted in index order while their blocks number at most max_blocks and
+    their staging bytes (each block's length rounded up to 16) take at most stage_bytes; the others get
+    ERROR_allocation_failed.  Arguments, n_frames and `stream` as for decompress_frames_async.  Returns nothing: read d_result
+    after the stream's work."""
+    ptr, n_frames, stream = _async_frame_args([d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_cap, d_result], n_frames,
+                                              stream)
+    _check(lib().LizardB200_compressFramesAsync(*ptr, n_frames, ctypes.byref(prefs) if prefs is not None else None, max_blocks,
+                                                stage_bytes, stream or None), "LizardB200_compressFramesAsync")
 
 
 def frame_error(result: int):

@@ -10,6 +10,7 @@
 #include "encode_dict_kernel.cuh"
 #include "frame_device_kernels.cuh"
 #include "frame_async_kernels.cuh"
+#include "frame_compress_async_kernels.cuh"
 
 #include <cuda_runtime.h>
 #include <mutex>
@@ -234,6 +235,7 @@ struct Context {
     DeviceBuffer d_in, d_out, d_tab, d_pack;
     DeviceBuffer fd_tab, fd_stage;            // tables and staged blocks of the device-memory frame calls (frame.inl)
     DeviceBuffer fa_tab, fa_stage;            // the same for LizardB200_decompressFramesAsync, kept apart: a captured graph holds them
+    DeviceBuffer fc_tab, fc_stage;            // and for LizardB200_compressFramesAsync, apart from both for the same reason
     EncodeConfig enc_cfg;
 };
 Context g_ctx[kMaxDevices];

@@ -279,4 +279,126 @@ LZ_HD u32 frame_settle_entries(const FrameInfoRec& fi, const FrameBlockRec* bloc
     return frame_settle_end(fi, cap, &st, check_hash);
 }
 
+// ---- LizardF_compressFrame's decisions for one frame --------------------------------------------------------------------------
+// The one statement of the frame header and the compression bounds: the host frame API (frame.inl: LizardF_compressBound,
+// LizardF_compressFrameBound, LizardF_compressBegin, LizardF_compressFrame, LizardB200_compressFrames) and the planning kernels
+// of LizardB200_compressFramesAsync (DESIGN.md 3.4c) run these functions.  Reference: lib/lizard_frame.c:231-312, :363-451.
+constexpr u32 kFwCompressionLevel = 5;                                      // LizardF_ERROR_compressionLevel_invalid
+// The LizardF_preferences_t fields the header and the bounds read, with the caller's enum values as they are (the enums'
+// underlying type is unsigned)
+struct FramePrefs { u32 bsid, block_mode, ccksum, auto_flush; u64 content_size; };
+
+// frame.inl's frame_block_size: the block size of an ID, 0 counting as 1; an invalid ID gives LizardF_ERROR_maxBlockSize_invalid
+// as a size_t, which the bounds below use as a size like the host code always has
+LZ_HD u64 frame_block_size_of(u32 bsid)
+{
+    const u32 b = frame_block_bytes(bsid == 0 ? 1u : bsid);
+    return b ? (u64)b : 0ull - kFwMaxBlockSize;
+}
+// the smallest block size ID from 128 KiB up to the requested one whose blocks hold the whole input (lizard_frame.c:231-240)
+LZ_HD u32 frame_optimal_bsid(u32 req, u64 src_size)
+{
+    int prop = 1;
+    while ((int)req > prop) {
+        if (src_size <= frame_block_size_of((u32)prop)) return (u32)prop;
+        prop++;
+    }
+    return req;
+}
+// LizardF_compressBound (lizard_frame.c:436-451)
+LZ_HD u64 frame_compress_bound(u64 src_size, const FramePrefs& p)
+{
+    const u64 bs = frame_block_size_of(p.bsid);
+    const u32 nb = (u32)(src_size / bs) + 1;
+    const u64 last = p.auto_flush ? src_size % bs : bs;
+    return 4 * (u64)nb + bs * (nb - 1) + last + 4 + (u64)p.ccksum * 4;
+}
+// LizardF_compressFrameBound (lizard_frame.c:242-247): a header of at most 15 bytes in front
+LZ_HD u64 frame_compress_frame_bound(u64 src_size, FramePrefs p)
+{
+    p.bsid = frame_optimal_bsid(p.bsid, src_size);
+    p.auto_flush = 1;
+    return 15 + frame_compress_bound(src_size, p);
+}
+// the preferences LizardF_compressFrame runs a frame of src_size bytes with (lizard_frame.c:260-290): the content size is the
+// input's if any is asked for (so none on an empty input), the optimal block size, autoFlush, and a frame of one block
+// independent whatever its preferences say
+LZ_HD FramePrefs frame_one_shot(FramePrefs p, u64 src_size)
+{
+    if (p.content_size != 0) p.content_size = src_size;
+    p.bsid = frame_optimal_bsid(p.bsid, src_size);
+    p.auto_flush = 1;
+    if (src_size <= frame_block_size_of(p.bsid)) p.block_mode = 1;
+    return p;
+}
+// LizardF_compressBegin's checks, in its order, and the header it writes to hdr (at most 15 bytes; nothing on an error): block
+// size ID (0 counts as 1), block mode, level (level_ok: the level the preferences give passes the GPU's level gate).  Returns
+// kFwOk or the error; *block_size and *hdr_len as the host call sets them.
+LZ_HD u32 frame_begin(const FramePrefs& p, bool level_ok, u8* hdr, u32* hdr_len, u64* block_size)
+{
+    const u32 bsid = p.bsid == 0 ? 1u : p.bsid;
+    *hdr_len = 0;
+    *block_size = frame_block_size_of(bsid);
+    if (!frame_block_bytes(bsid)) return kFwMaxBlockSize;
+    if (p.block_mode != 1) return kFwBlockMode;
+    if (!level_ok) return kFwCompressionLevel;
+    wr_le32(hdr, 0x184D2206u);
+    hdr[4] = (u8)((1u << 6) + ((p.block_mode & 1) << 5) + ((p.ccksum & 1) << 2) + ((p.content_size > 0) << 3));
+    hdr[5] = (u8)((bsid & 7) << 4);
+    u32 n = 6;
+    if (p.content_size) { wr_le32(hdr + 6, (u32)p.content_size); wr_le32(hdr + 10, (u32)(p.content_size >> 32)); n = 14; }
+    hdr[n] = (u8)(xxh32_serial(hdr + 4, n - 4, 0) >> 8);
+    *hdr_len = n + 1;
+    return kFwOk;
+}
+
+// What LizardF_compressFrame decides about one frame before it compresses anything
+struct FrameCompressPlan {
+    u32 verdict;          // kFwOk; kFwDstTooSmall below LizardF_compressFrameBound; else LizardF_compressBegin's error
+    u32 hdr_len;
+    u32 ccksum;           // the frame ends with the content checksum
+    u32 block_size;
+    u64 n_blocks;         // blocks of block_size, the last one shorter
+    u64 stage;            // the blocks' lengths, each rounded up to 16: the encoder's output slots
+};
+// The frame of src_size bytes with cap bytes of room, under the caller's preferences; the header goes to hdr (16 bytes of room).
+LZ_HD void frame_compress_plan(const FramePrefs& prefs, bool level_ok, u64 src_size, u64 cap, u8* hdr, FrameCompressPlan* pl)
+{
+    pl->hdr_len = 0; pl->ccksum = 0; pl->block_size = 0; pl->n_blocks = 0; pl->stage = 0;
+    const FramePrefs p = frame_one_shot(prefs, src_size);
+    if (cap < frame_compress_frame_bound(src_size, p)) { pl->verdict = kFwDstTooSmall; return; }
+    u64 bs;
+    pl->verdict = frame_begin(p, level_ok, hdr, &pl->hdr_len, &bs);
+    if (pl->verdict != kFwOk) return;
+    pl->ccksum = p.ccksum == 1;
+    pl->block_size = (u32)bs;
+    pl->n_blocks = src_size / bs + (src_size % bs != 0);
+    if (pl->n_blocks) pl->stage = (pl->n_blocks - 1) * bs + ((src_size - (pl->n_blocks - 1) * bs + 15) & ~15ull);
+}
+
+// LizardB200_compressFramesAsync's admission: a prefix over frames in index order.  Frame i is admitted while the blocks of
+// frames 0..i number at most max_blocks and their staging bytes stay within stage_bytes (frame_admit_blocks and
+// frame_admit_slots on the two exclusive sums).  A frame that fails its checks, and an empty one, take nothing.  A frame's
+// blocks count as at most max_blocks + 1, which decides the same and keeps the sum over 2^32 frames from wrapping.
+LZ_HD u64 frame_compress_demand_blocks(const FrameCompressPlan& pl, u32 max_blocks)
+{
+    if (pl.verdict != kFwOk) return 0;
+    return pl.n_blocks <= max_blocks ? pl.n_blocks : (u64)max_blocks + 1;
+}
+LZ_HD u64 frame_compress_demand_stage(const FrameCompressPlan& pl) { return pl.verdict == kFwOk ? pl.stage : 0; }
+// the largest block a frame of these preferences can have: the preferences' block size, 256 MiB for an invalid ID (which
+// frame_optimal_bsid may map to any valid one)
+LZ_HD u64 frame_compress_top_block(u32 bsid)
+{
+    const u32 b = frame_block_bytes(bsid == 0 ? 1u : bsid);
+    return b ? b : frame_block_bytes(7);
+}
+// The staging bytes a call can ever use: max_blocks blocks of the top block size.  A larger stage_bytes, up to SIZE_MAX for
+// "no bound", admits the same frames, so the call sizes its arena by this and never by more.
+LZ_HD u64 frame_compress_stage_limit(u32 max_blocks, u32 bsid, u64 stage_bytes)
+{
+    const u64 most = (u64)max_blocks * frame_compress_top_block(bsid);
+    return stage_bytes < most ? stage_bytes : most;
+}
+
 }  // namespace lzb

@@ -924,3 +924,45 @@ extern "C" unsigned long long lzb_host_frame_async_decode(const unsigned char* s
     if (v != lzb::kFwOk) return (unsigned long long)-(long long)v;
     return fi.skippable ? 0 : out;
 }
+
+// LizardB200_compressFramesAsync's per-frame decisions (frame_device.cuh: frame_compress_plan) for a frame of src bytes with
+// cap bytes of room under the given preference fields.  Returns the verdict; hdr (16 bytes) gets the header, out[0..4] the
+// header length, block size, block count, staging bytes and checksum flag.
+extern "C" unsigned lzb_host_frame_compress_plan(unsigned bsid, unsigned block_mode, unsigned ccksum, unsigned auto_flush,
+                                                 unsigned long long content_size, int level_ok, unsigned long long src,
+                                                 unsigned long long cap, unsigned char* hdr, unsigned long long* out)
+{
+    const lzb::FramePrefs p{ bsid, block_mode, ccksum, auto_flush, content_size };
+    lzb::FrameCompressPlan pl;
+    lzb::frame_compress_plan(p, level_ok != 0, src, cap, hdr, &pl);
+    out[0] = pl.hdr_len; out[1] = pl.block_size; out[2] = pl.n_blocks; out[3] = pl.stage; out[4] = pl.ccksum;
+    return pl.verdict;
+}
+
+// the staging arena LizardB200_compressFramesAsync sizes for (max_blocks, the preferences' block size ID, stage_bytes)
+extern "C" unsigned long long lzb_host_frame_compress_stage_limit(unsigned max_blocks, unsigned bsid, unsigned long long stage_bytes)
+{
+    return lzb::frame_compress_stage_limit(max_blocks, bsid, stage_bytes);
+}
+
+// LizardB200_compressFramesAsync's planning (frame_compress_async_kernels.cuh) serially over n frames of sizes[i] bytes with
+// caps[i] bytes of room: the plan of each frame, its demands and the admission on the two exclusive sums, after the stage
+// clamp.  Writes adm[i], the block base first[i] and the staging base sbase[i].
+extern "C" void lzb_host_frame_compress_admit(unsigned n, const unsigned long long* sizes, const unsigned long long* caps,
+                                              unsigned bsid, unsigned block_mode, unsigned ccksum, unsigned long long content_size,
+                                              int level_ok, unsigned max_blocks, unsigned long long stage_bytes, unsigned* adm,
+                                              unsigned long long* first, unsigned long long* sbase)
+{
+    const lzb::FramePrefs p{ bsid, block_mode, ccksum, 0, content_size };
+    stage_bytes = lzb::frame_compress_stage_limit(max_blocks, bsid, stage_bytes);
+    lzb::u64 bb = 0, sb = 0;
+    unsigned char hdr[16];
+    for (unsigned i = 0; i < n; ++i) {
+        lzb::FrameCompressPlan pl;
+        lzb::frame_compress_plan(p, level_ok != 0, sizes[i], caps[i], hdr, &pl);
+        const lzb::u64 b = lzb::frame_compress_demand_blocks(pl, max_blocks), s = lzb::frame_compress_demand_stage(pl);
+        adm[i] = lzb::frame_admit_blocks(bb, b, max_blocks) && lzb::frame_admit_slots(sb, s, stage_bytes);
+        first[i] = bb; sbase[i] = sb;
+        bb += b; sb += s;
+    }
+}
