@@ -354,6 +354,34 @@ int LizardB200_compressFramesAsync(const void* dSrc, const uint64_t* dSrcOff, co
                                    void* dDst, const uint64_t* dDstOff, const uint64_t* dDstCap,
                                    size_t* dResult, unsigned nFrames, const LizardF_preferences_t* prefs,
                                    unsigned maxBlocks, size_t stageBytes, void* cudaStream);
+/* Streaming decompression of LizardF data held in device memory (DESIGN.md 3.4d): LizardF_decompress on device buffers.
+ * A stream is bound to the device current when it is created; create and free return LIZARDB200_OK or an error status.
+ * LizardB200_decompressStream takes device pointers dSrc / dDst and host pointers srcSizePtr / dstSizePtr.  For any sequence of
+ * calls, each call returns what this library's LizardF_decompress returns when a fresh context is handed host copies of the
+ * same chunks and capacities in the same order: the hint or error code, *srcSizePtr, *dstSizePtr and the bytes in
+ * [dDst, dDst + *dstSizePtr).  Its rules all carry over: skippable frames, concatenated frames (a call ends at the end of a
+ * frame, hint 0), LizardF_ERROR_srcPtr_wrong when dSrc is not where the previous call stopped while it left input unconsumed,
+ * LizardF_ERROR_blockMode_invalid for linked blocks.  Nothing is written outside [dDst, dDst + *dstSizePtr on entry); bytes
+ * behind the produced size are unspecified, as on the host.  The stream keeps the carried bytes of an incomplete block and a
+ * one-block output buffer in device memory (up to the frame's maximum block size each, allocated when a header names it and
+ * freed with the stream) and the running content checksum.
+ * The call waits for earlier work on `cudaStream`, works on it (workspace hand-over between streams as for the other device
+ * calls) and synchronises it before it returns, because it returns sizes: it is neither enqueue-only nor capturable.  A chunk
+ * of many complete blocks costs a fixed number of launches whatever it holds: a walk over the block records, one decode of the
+ * compressed blocks (at most 1 GiB of staging slots of the maximum block size per round; blocks decoding far below that size
+ * can take further rounds), one placement and, with the content checksum, one checksum launch.  The checksum runs on one
+ * warp, about 0.7 GB/s on an H100 (DESIGN.md 3.4d), which bounds a checksummed stream: there the host LizardF_decompress is
+ * faster.  Device memory: the staging arena of a round is the device context's, shared by its streams and kept until the
+ * process ends; it holds one slot of the maximum block size per decode unit, up to 1 GiB + one block (plus the allocator's
+ * 25% when it grows) after a call with a large chunk into a large output, e.g. about 1.25 GiB for 64 MiB chunks of 128 KiB
+ * blocks and about 1.6 GiB for frames of 256 MiB blocks; the units are bounded by the output's room too.  After
+ * LizardF_ERROR_contentChecksum_invalid the stream is where the host context is after that error, so further calls still
+ * answer alike.  A CUDA failure gives LizardF_ERROR_GENERIC, no device memory LizardF_ERROR_allocation_failed. */
+typedef struct LizardB200_dstream_s LizardB200_dstream_t;
+int LizardB200_createDecompressionStream(LizardB200_dstream_t** out);
+int LizardB200_freeDecompressionStream(LizardB200_dstream_t* ds);
+size_t LizardB200_decompressStream(LizardB200_dstream_t* ds, void* dDst, size_t* dstSizePtr,
+                                   const void* dSrc, size_t* srcSizePtr, void* cudaStream);
 /* diagnostics: launch shape of the encode kernel for a level (no device needed): warps per CTA, how many of them keep their
  * hash table in shared memory, CTAs per SM (an upper bound: a launch holds no more than fit), dynamic shared memory per CTA.
  * The level's default, or LIZARDB200_ENC_SHAPE="warps,tables,ctas" when that is set and valid, exactly as the encoder

@@ -39,6 +39,11 @@ def lib():
         L.Lizard_compress_extState.argtypes = [ctypes.c_void_p] + L.Lizard_compress.argtypes
         L.Lizard_decompress_safe.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
         L.LizardB200_lastError.restype = ctypes.c_char_p
+        L.LizardB200_createDecompressionStream.argtypes = [ctypes.POINTER(ctypes.c_void_p)]
+        L.LizardB200_freeDecompressionStream.argtypes = [ctypes.c_void_p]
+        L.LizardB200_decompressStream.restype = ctypes.c_size_t
+        L.LizardB200_decompressStream.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_size_t),
+                                                  ctypes.c_void_p, ctypes.POINTER(ctypes.c_size_t), ctypes.c_void_p]
         L.LizardB200_launchCount.restype = ctypes.c_ulonglong
         L.LizardB200_compress_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int, ctypes.c_int]
         L.LizardB200_decompress_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int]
@@ -393,10 +398,7 @@ def decompress_frames(d_src: int, src_off, src_size, d_dst: int, dst_off, dst_ca
 def _async_frame_args(args, n_frames, stream):
     """The device addresses, n_frames and stream of a device-table frame call: args are the source, its offset and size tables,
     the destination, its offset and capacity tables and the results, each a device address as an integer or a CUDA tensor."""
-    tensors = [a for a in args if not isinstance(a, int)]
-    for a in tensors:
-        if not (a.is_cuda and a.is_contiguous()):
-            raise ValueError("tensor arguments must be contiguous CUDA tensors")
+    ptr, stream = _device_args(args, stream)
     tables = [a for a in args[1:3] + args[4:] if not isinstance(a, int)]
     for a in tables:
         if a.element_size() != 8:
@@ -408,6 +410,16 @@ def _async_frame_args(args, n_frames, stream):
     for a in tables:
         if a.numel() < n_frames:
             raise ValueError("a table holds fewer entries than n_frames")
+    return ptr, n_frames, stream
+
+
+def _device_args(args, stream):
+    """The device addresses of args (integers, or contiguous CUDA tensors) and the stream: None means the current torch stream
+    of the first tensor, or 0 (the default stream) when every argument is an address."""
+    tensors = [a for a in args if not isinstance(a, int)]
+    for a in tensors:
+        if not (a.is_cuda and a.is_contiguous()):
+            raise ValueError("tensor arguments must be contiguous CUDA tensors")
     if stream is None:
         if tensors:
             import torch
@@ -416,7 +428,7 @@ def _async_frame_args(args, n_frames, stream):
             stream = 0
     elif not isinstance(stream, int):
         stream = stream.cuda_stream
-    return [a if isinstance(a, int) else a.data_ptr() for a in args], n_frames, stream
+    return [a if isinstance(a, int) else a.data_ptr() for a in args], stream
 
 
 def decompress_frames_async(d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_cap, d_result, max_blocks: int,
@@ -445,6 +457,43 @@ def compress_frames_async(d_src, d_src_off, d_src_size, d_dst, d_dst_off, d_dst_
                                               stream)
     _check(lib().LizardB200_compressFramesAsync(*ptr, n_frames, ctypes.byref(prefs) if prefs is not None else None, max_blocks,
                                                 stage_bytes, stream or None), "LizardB200_compressFramesAsync")
+
+
+class DecompressionStream:
+    """LizardB200_decompressStream: LizardF_decompress over device memory, one chunk per call, with its state kept between
+    calls on the device current at creation (include/lizard_b200.h).  Use close() or a `with` block to free it."""
+
+    def __init__(self):
+        self._ds = ctypes.c_void_p()
+        _check(lib().LizardB200_createDecompressionStream(ctypes.byref(self._ds)), "LizardB200_createDecompressionStream")
+
+    def decompress(self, d_src, src_size: int, d_dst, dst_cap: int, stream=None):
+        """Feed the src_size bytes at d_src with room for dst_cap bytes at d_dst (device addresses as integers, or contiguous
+        CUDA tensors); `stream` as for decompress_frames_async (the current torch stream when tensors are given, else 0).  Returns (hint, consumed, produced): hint is LizardF_decompress's
+        return value (a size_t; frame_error names an error)."""
+        if self._ds is None:
+            raise ValueError("the stream is closed")
+        (src, dst), stream = _device_args([d_src, d_dst], stream)
+        ss, ds = ctypes.c_size_t(src_size), ctypes.c_size_t(dst_cap)
+        hint = lib().LizardB200_decompressStream(self._ds, dst, ctypes.byref(ds), src, ctypes.byref(ss), stream or None)
+        return hint, ss.value, ds.value
+
+    def close(self):
+        if self._ds is not None:
+            lib().LizardB200_freeDecompressionStream(self._ds)
+            self._ds = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def frame_error(result: int):

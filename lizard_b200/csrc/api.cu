@@ -11,6 +11,8 @@
 #include "frame_device_kernels.cuh"
 #include "frame_async_kernels.cuh"
 #include "frame_compress_async_kernels.cuh"
+#include "frame_stream_kernels.cuh"
+#include "frame_stream.h"
 
 #include <cuda_runtime.h>
 #include <mutex>
@@ -236,6 +238,7 @@ struct Context {
     DeviceBuffer fd_tab, fd_stage;            // tables and staged blocks of the device-memory frame calls (frame.inl)
     DeviceBuffer fa_tab, fa_stage;            // the same for LizardB200_decompressFramesAsync, kept apart: a captured graph holds them
     DeviceBuffer fc_tab, fc_stage;            // and for LizardB200_compressFramesAsync, apart from both for the same reason
+    DeviceBuffer ds_tab, ds_stage, ds_seg;    // a LizardB200_decompressStream round's tables and staged blocks, its segment lists
     EncodeConfig enc_cfg;
 };
 Context g_ctx[kMaxDevices];

@@ -401,4 +401,67 @@ LZ_HD u64 frame_compress_stage_limit(u32 max_blocks, u32 bsid, u64 stage_bytes)
     return stage_bytes < most ? stage_bytes : most;
 }
 
+// ---- LizardB200_decompressStream (DESIGN.md 3.4d): the block walk of one chunk, and the running content checksum ------------
+// One record per size word the walk reads: where it is (from the walk's first byte), the word, and the decode unit of a
+// complete compressed block (-1: no unit).  The last record of a walk that stops on a word is that word.
+struct StreamWalkRec { u64 pos; u32 word; int unit; };
+enum : u32 { kWalkShort = 0,        // fewer than 4 bytes left for the next size word
+             kWalkEnd = 1,          // the end mark (the last record)
+             kWalkBadSize = 2,      // a size word above the maximum block size (the last record)
+             kWalkPartial = 3,      // a block whose payload is not all there (the last record)
+             kWalkRecords = 4,      // the record table is full
+             kWalkSlots = 5 };      // a complete compressed block found no decode unit (the last record, unit -1)
+// tail: up to 8 bytes behind the end mark (the content checksum), little-endian, tail_n of them present
+struct StreamWalk { u32 n_recs, stop, n_units, tail_n; u64 tail; };
+// `len` bytes at address src, placed at address dst (the checksum's pieces leave dst 0)
+struct StreamSeg { u64 src, dst, len; };
+// The records of the n bytes at p, which start on a size word, with frame_walk's checks: at most max_recs records, and
+// compressed blocks take decode units 1..slots (unit 0 is the carried block's) with u_src the payload's address and u_len its
+// size.  Serial: one thread.
+LZ_HD StreamWalk frame_stream_walk(const u8* p, u64 n, u32 max_block, StreamWalkRec* rec, u32 max_recs, u32 slots, u64* u_src,
+                                   u32* u_len)
+{
+    StreamWalk w = { 0, kWalkShort, 0, 0, 0 };
+    u64 pos = 0;
+    for (;;) {
+        if (n - pos < 4) { w.stop = kWalkShort; break; }
+        if (w.n_recs == max_recs) { w.stop = kWalkRecords; break; }
+        const u32 word = rd_le32(p + pos), csz = word & 0x7FFFFFFFu;
+        StreamWalkRec& r = rec[w.n_recs++];
+        r.pos = pos; r.word = word; r.unit = -1;
+        if (csz == 0) {
+            w.stop = kWalkEnd;
+            for (u64 k = pos + 4; k < n && w.tail_n < 8; ++k) w.tail |= (u64)p[k] << (8 * w.tail_n++);
+            break;
+        }
+        if (csz > max_block) { w.stop = kWalkBadSize; break; }
+        if (n - pos - 4 < csz) { w.stop = kWalkPartial; break; }
+        if (!(word >> 31)) {
+            if (w.n_units == slots) { w.stop = kWalkSlots; break; }
+            r.unit = (int)++w.n_units;
+            u_src[w.n_units] = (u64)(size_t)(p + pos + 4); u_len[w.n_units] = csz;
+        }
+        pos += 4 + csz;
+    }
+    return w;
+}
+
+// XXH32 (seed 0) over bytes that arrive in pieces: the four accumulators, the length so far and the bytes short of a stripe
+struct StreamHashState { u32 v[4]; u64 total; u32 nbuf, pad; u8 buf[16]; };
+LZ_HD void xx_stream_reset(StreamHashState* s)
+{
+    for (u32 l = 0; l < 4; ++l) s->v[l] = xx_lane_init(0, l);
+    s->total = 0; s->nbuf = 0; s->pad = 0;
+    for (u32 i = 0; i < 16; ++i) s->buf[i] = 0;
+}
+LZ_HD void xx_stream_update(StreamHashState* s, const u8* p, u64 n)
+{
+    s->total += n;
+    while (n) {
+        s->buf[s->nbuf++] = *p++; --n;
+        if (s->nbuf == 16) { for (u32 l = 0; l < 4; ++l) s->v[l] = xx_round(s->v[l], rd_le32(s->buf + 4 * l)); s->nbuf = 0; }
+    }
+}
+LZ_HD u32 xx_stream_digest(const StreamHashState* s) { return xx_finish(s->v, s->total, s->buf, s->nbuf, 0); }
+
 }  // namespace lzb

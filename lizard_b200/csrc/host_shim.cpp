@@ -966,3 +966,84 @@ extern "C" void lzb_host_frame_compress_admit(unsigned n, const unsigned long lo
         bb += b; sb += s;
     }
 }
+
+// ---- LizardB200_decompressStream on the host (frame_stream.h): the state machine and StreamIO over host memory, the walk
+// and the one-lane decoder standing in for the kernels, so the CPU tests compare a stream call for call with the reference.
+#include "frame_stream.h"
+namespace {
+struct HostStreamExec {
+    std::vector<lzb::u8> stage;
+    lzb::u64 rounds = 0;
+    void read(void* to, const void* p, size_t n) { memcpy(to, p, n); }
+    void copy(void* to, const void* from, size_t n) { memmove(to, from, n); }
+    void sync() {}
+    void round(const lzb::u8* p, lzb::u64 n, lzb::u32 mb, const lzb::u8* carry, lzb::u32 carry_len, lzb::u32 max_recs,
+               lzb::u32 slots, lzb::StreamWalk* walk, lzb::StreamWalkRec* recs, int* res, lzb::u8** st)
+    {
+        ++rounds;
+        const size_t U = (size_t)slots + 1;
+        std::vector<lzb::u64> u_src(U, 0);
+        std::vector<lzb::u32> u_len(U, 0);
+        *walk = lzb::frame_stream_walk(p, n, mb, recs, max_recs, slots, u_src.data(), u_len.data());
+        u_src[0] = (lzb::u64)(size_t)carry; u_len[0] = carry_len;
+        stage.assign(U * mb + 64, 0);
+        for (size_t k = 0; k < U; ++k)
+            res[k] = k <= walk->n_units ? lzb_host_decompress((const unsigned char*)(size_t)u_src[k], (int)u_len[k], stage.data() + k * mb, (int)mb) : 0;
+        *st = stage.data();
+    }
+    void gather(const std::vector<lzb::StreamSeg>& segs) { for (const lzb::StreamSeg& g : segs) memcpy((void*)(size_t)g.dst, (const void*)(size_t)g.src, g.len); }
+    void hash(const std::vector<lzb::StreamSeg>& segs, lzb::StreamHashState* h)
+    {
+        for (const lzb::StreamSeg& g : segs) lzb::xx_stream_update(h, (const lzb::u8*)(size_t)g.src, g.len);
+    }
+    void hash_reset(lzb::StreamHashState* h) { lzb::xx_stream_reset(h); }
+    lzb::u32 digest(lzb::StreamHashState* h) { return lzb::xx_stream_digest(h); }
+    void buffers(lzb::StreamBuffers& sb, size_t block)
+    {
+        if (block <= sb.block) return;
+        free(sb.carry); free(sb.tmp_out);
+        sb.carry = (lzb::u8*)malloc(block + 16); sb.tmp_out = (lzb::u8*)malloc(block + 64);
+        if (!sb.carry || !sb.tmp_out) throw std::bad_alloc();
+        sb.block = block; sb.tmp_at = sb.tmp_out;
+    }
+};
+struct HostStream { lzb::FrameDState d; lzb::StreamBuffers sb; lzb::StreamHashState h; HostStreamExec x; };
+}  // namespace
+
+extern "C" void* lzb_host_stream_new()
+{
+    HostStream* s = new HostStream();
+    s->d.reset();
+    s->sb.hash = &s->h;
+    lzb::xx_stream_reset(&s->h);
+    return s;
+}
+extern "C" void lzb_host_stream_free(void* p)
+{
+    HostStream* s = (HostStream*)p;
+    free(s->sb.carry); free(s->sb.tmp_out);
+    delete s;
+}
+// one LizardB200_decompressStream call; *rounds (if not null) gets the rounds (walk + decode) the call ran
+extern "C" size_t lzb_host_stream_call(void* p, unsigned char* dst, size_t* dst_size, const unsigned char* src, size_t* src_size,
+                                       unsigned long long* rounds)
+{
+    HostStream* s = (HostStream*)p;
+    const lzb::u64 r0 = s->x.rounds;
+    size_t r;
+    try { r = lzb::frame_stream_call(s->x, s->sb, &s->d, dst, dst_size, src, src_size); }
+    catch (const std::bad_alloc&) { r = lzb::ferr(lzb::FE_allocation_failed); }
+    if (rounds) *rounds = s->x.rounds - r0;
+    return r;
+}
+// the walk of one round (frame_stream_walk): records as (pos, word, unit) triples, and the summary (records, stop, units)
+extern "C" void lzb_host_stream_walk(const unsigned char* p, unsigned long long n, unsigned max_block, unsigned max_recs,
+                                     unsigned slots, unsigned long long* pos, unsigned* word, int* unit, unsigned* summary)
+{
+    std::vector<lzb::StreamWalkRec> rec(max_recs);
+    std::vector<lzb::u64> u_src((size_t)slots + 1);
+    std::vector<lzb::u32> u_len((size_t)slots + 1);
+    const lzb::StreamWalk w = lzb::frame_stream_walk(p, n, max_block, rec.data(), max_recs, slots, u_src.data(), u_len.data());
+    for (lzb::u32 i = 0; i < w.n_recs; ++i) { pos[i] = rec[i].pos; word[i] = rec[i].word; unit[i] = rec[i].unit; }
+    summary[0] = w.n_recs; summary[1] = w.stop; summary[2] = w.n_units;
+}
