@@ -382,6 +382,49 @@ int LizardB200_createDecompressionStream(LizardB200_dstream_t** out);
 int LizardB200_freeDecompressionStream(LizardB200_dstream_t* ds);
 size_t LizardB200_decompressStream(LizardB200_dstream_t* ds, void* dDst, size_t* dstSizePtr,
                                    const void* dSrc, size_t* srcSizePtr, void* cudaStream);
+/* Streaming compression into LizardF frames in device memory (DESIGN.md 3.4e): LizardF_compressBegin / Update / flush / End on
+ * device buffers, enqueue-only.  A stream is bound to the device current when it is created; create and free return
+ * LIZARDB200_OK or an error status.  dDst, dSrc and dWritten are device pointers; prefs, dstMax and srcSize host values;
+ * dWritten may be NULL.
+ * Same answers as the host API: for any sequence of calls, call k writes to *dWritten, in stream order, what this library's
+ * LizardF_compressBegin / LizardF_compressUpdate / LizardF_flush / LizardF_compressEnd return when a fresh context is handed
+ * host copies of the same preferences, chunks and capacities in the same order (a size or an error code), and writes the same
+ * bytes to [dDst, dDst + size).  That covers every refusal of the host calls: refused levels and linked blocks at Begin,
+ * dstMax below LizardF_compressBound, the flush's capacity check, calls in the wrong stage, and the contentSize check at End,
+ * which writes the end mark and the checksum first and then the error code to *dWritten, as the host call returns it.  One
+ * difference: with autoFlush, no content checksum and dstMax exactly LizardF_compressBound, an Update whose last block is 1 byte
+ * long (its record is 10 bytes, 5 more than the bound counts) and whose other blocks all are stored raw does not fit; the host
+ * call writes records up to its capacity and returns ERROR_dstMaxSize_tooSmall, keeping its total, while the device call
+ * writes ERROR_dstMaxSize_tooSmall to *dWritten and its stream goes on as after a call that fitted.
+ * A new stream answers as a fresh host context does, also before any successful Begin.
+ * Host return value: the error code when the host call's result is an error, which every error here can be decided on the host;
+ * otherwise 0, "enqueued".  A call refused before it does any work enqueues nothing, leaves *dWritten unwritten and leaves the
+ * stream where the host context would be.
+ * Enqueue-only: a call that does not grow a buffer issues no host<->device copy, no allocation and no synchronisation, and its
+ * launches depend only on its host arguments and the stream's host state.  Growing synchronises `cudaStream`: the first Begin
+ * for a block size (the carried block) and an Update larger than any before it, up to the round bound (a round's block table and
+ * encoder slots).  Inside a capture a call that would have to grow returns LizardF_ERROR_GENERIC (LizardB200_lastError says
+ * why), enqueues nothing and leaves the stream unchanged.  After one uncaptured run of the same sizes, a Begin, Update..., Flush,
+ * End sequence can be captured in a CUDA graph; each replay writes a complete frame of what the source buffers then hold
+ * (Begin's kernel resets the device-side state).
+ * Streams: the calls on one stream object must be on one CUDA stream, or ordered by the caller (its device state is read and
+ * written in stream order).  The encoder's workspace is shared by the device's calls with the hand-over of the other device calls.
+ * Device memory per stream, kept until it is freed: the carried partial block (one block of the frame's block size: up to
+ * 256 MiB at block size ID 7), the running XXH32 state and the call's record offset, and a round's block table and encoder slots
+ * (a round takes at most 1 GiB of blocks, at least one block: for 128 KiB blocks up to 8192 blocks and 1 GiB; a chunk of more
+ * blocks runs several rounds, each with the same launches).  An Update enqueues: a device-to-device copy completing the carried
+ * block, per round a planning kernel, the encoder, a scan and an assembly kernel, with the content checksum one checksum
+ * kernel over the chunk, a device-to-device copy of the remainder to the carried block, and a result kernel.  The checksum runs
+ * on one warp, about 0.7 GB/s on an H100 (DESIGN.md 3.4d), which bounds a checksummed stream. */
+typedef struct LizardB200_cstream_s LizardB200_cstream_t;
+int    LizardB200_createCompressionStream(LizardB200_cstream_t** out);
+int    LizardB200_freeCompressionStream(LizardB200_cstream_t* cs);
+size_t LizardB200_compressStreamBegin (LizardB200_cstream_t* cs, void* dDst, size_t dstMax,
+                                       const LizardF_preferences_t* prefs, size_t* dWritten, void* cudaStream);
+size_t LizardB200_compressStreamUpdate(LizardB200_cstream_t* cs, void* dDst, size_t dstMax,
+                                       const void* dSrc, size_t srcSize, size_t* dWritten, void* cudaStream);
+size_t LizardB200_compressStreamFlush (LizardB200_cstream_t* cs, void* dDst, size_t dstMax, size_t* dWritten, void* cudaStream);
+size_t LizardB200_compressStreamEnd   (LizardB200_cstream_t* cs, void* dDst, size_t dstMax, size_t* dWritten, void* cudaStream);
 /* diagnostics: launch shape of the encode kernel for a level (no device needed): warps per CTA, how many of them keep their
  * hash table in shared memory, CTAs per SM (an upper bound: a launch holds no more than fit), dynamic shared memory per CTA.
  * The level's default, or LIZARDB200_ENC_SHAPE="warps,tables,ctas" when that is set and valid, exactly as the encoder

@@ -45,6 +45,15 @@ def lib():
         L.LizardB200_decompressStream.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_size_t),
                                                   ctypes.c_void_p, ctypes.POINTER(ctypes.c_size_t), ctypes.c_void_p]
         L.LizardB200_launchCount.restype = ctypes.c_ulonglong
+        vp, sz = ctypes.c_void_p, ctypes.c_size_t
+        L.LizardB200_createCompressionStream.argtypes = [ctypes.POINTER(vp)]
+        L.LizardB200_freeCompressionStream.argtypes = [vp]
+        L.LizardB200_compressStreamBegin.argtypes = [vp, vp, sz, vp, vp, vp]
+        L.LizardB200_compressStreamUpdate.argtypes = [vp, vp, sz, vp, sz, vp, vp]
+        L.LizardB200_compressStreamFlush.argtypes = [vp, vp, sz, vp, vp]
+        L.LizardB200_compressStreamEnd.argtypes = [vp, vp, sz, vp, vp]
+        for f in ("Begin", "Update", "Flush", "End"):
+            getattr(L, "LizardB200_compressStream" + f).restype = sz
         L.LizardB200_compress_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int, ctypes.c_int]
         L.LizardB200_decompress_batch.argtypes = [vpp, c_int_p, vpp, c_int_p, c_int_p, ctypes.c_int]
         L.Lizard_decompress_safe_partial.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -482,6 +491,73 @@ class DecompressionStream:
         if self._ds is not None:
             lib().LizardB200_freeDecompressionStream(self._ds)
             self._ds = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class CompressionStream:
+    """LizardB200_compressStream*: LizardF_compressBegin / Update / flush / End over device memory, with the stream's state kept
+    between calls on the device current at creation (include/lizard_b200.h).  Addresses are integers or contiguous CUDA tensors;
+    `stream` as for decompress_frames_async.  With d_written=None a method synchronises the stream and returns the call's result
+    (a size or a LizardF error code, see frame_error); with a device address (8 bytes) it only enqueues and returns the host
+    return value (0, or the error code of a refused call).  Use close() or a `with` block to free it."""
+
+    def __init__(self):
+        L = lib()
+        self._cs = ctypes.c_void_p()
+        _check(L.LizardB200_createCompressionStream(ctypes.byref(self._cs)), "LizardB200_createCompressionStream")
+
+    def _call(self, fn, addrs, d_written, stream, args):
+        """fn(stream object, *args(device addresses of addrs), dWritten, cudaStream)"""
+        if self._cs is None:
+            raise ValueError("the stream is closed")
+        import torch
+        own = None
+        if d_written is None:
+            t = next((a for a in addrs if not isinstance(a, int)), None)
+            own = torch.empty(1, dtype=torch.int64, device=t.device if t is not None else "cuda")
+        ptr, stream = _device_args(addrs + [d_written if own is None else own], stream)
+        r = fn(self._cs, *args(ptr), ptr[-1], stream or None)
+        if own is None or lib().LizardF_isError(r):
+            return r
+        if stream:
+            torch.cuda.ExternalStream(stream).synchronize()
+        else:
+            torch.cuda.synchronize(own.device)
+        return int(own.item()) & ((1 << 64) - 1)
+
+    def begin(self, d_dst, dst_cap: int, prefs, d_written=None, stream=None):
+        """LizardF_compressBegin: the frame header for `prefs` (a Preferences, make_prefs; None = zeroed) at d_dst."""
+        p = ctypes.byref(prefs) if prefs is not None else None
+        return self._call(lib().LizardB200_compressStreamBegin, [d_dst], d_written, stream, lambda a: (a[0], dst_cap, p))
+
+    def update(self, d_src, src_size: int, d_dst, dst_cap: int, d_written=None, stream=None):
+        """LizardF_compressUpdate: the src_size bytes at d_src, records to d_dst with room for dst_cap bytes."""
+        return self._call(lib().LizardB200_compressStreamUpdate, [d_dst, d_src], d_written, stream,
+                          lambda a: (a[0], dst_cap, a[1], src_size))
+
+    def flush(self, d_dst, dst_cap: int, d_written=None, stream=None):
+        """LizardF_flush: the carried partial block as a record."""
+        return self._call(lib().LizardB200_compressStreamFlush, [d_dst], d_written, stream, lambda a: (a[0], dst_cap))
+
+    def end(self, d_dst, dst_cap: int, d_written=None, stream=None):
+        """LizardF_compressEnd: flush, the end mark and the content checksum."""
+        return self._call(lib().LizardB200_compressStreamEnd, [d_dst], d_written, stream, lambda a: (a[0], dst_cap))
+
+    def close(self):
+        if self._cs is not None:
+            lib().LizardB200_freeCompressionStream(self._cs)
+            self._cs = None
 
     def __enter__(self):
         return self

@@ -13,6 +13,8 @@
 #include "frame_compress_async_kernels.cuh"
 #include "frame_stream_kernels.cuh"
 #include "frame_stream.h"
+#include "frame_cstream_kernels.cuh"
+#include "frame_cstream.h"
 
 #include <cuda_runtime.h>
 #include <mutex>

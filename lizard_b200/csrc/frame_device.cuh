@@ -68,6 +68,16 @@ struct FrameBlockRec {
     u32 raw;              // 1 = stored block
 };
 
+// A frame block record's payload size for a block of len bytes that compressed to r (0 = did not fit len - 1 bytes): the
+// compressed bytes, or the raw block.  A 1-byte block becomes the 6-byte raw inner block the reference produces through its
+// wrapped bound check (lizard_frame.c:459 capacity 0, lizard_compress.c:238), written by frame_one_byte_record.
+LZ_HD u32 frame_record_payload(u32 len, int r) { return len == 1 ? 6u : (r > 0 ? (u32)r : len); }
+LZ_HD void frame_one_byte_record(u8* o, int level, u8 byte)
+{
+    o[0] = 6; o[1] = 0; o[2] = 0; o[3] = 0;
+    o[4] = (u8)level; o[5] = (u8)kFlagRaw; o[6] = 1; o[7] = 0; o[8] = 0; o[9] = byte;
+}
+
 // maximum block size of a block size ID (lib/lizard_frame.c:194), 0 for an invalid one; frame.inl's frame_block_size too
 LZ_HD u32 frame_block_bytes(u32 bsid)
 {

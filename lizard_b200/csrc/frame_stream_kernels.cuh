@@ -27,12 +27,12 @@ __global__ void __launch_bounds__(128) lizard_frame_stream_walk_kernel(const u8*
     }
 }
 
-// The stream's content checksum over n segments in order, on one warp: the warp stages up to kHashPiece bytes behind the
+// A stream's content checksum over n segments in order, on one warp: the warp stages up to kHashPiece bytes behind the
 // bytes short of a stripe (aligned 16-byte loads), lanes 0-3 run the four accumulators over the whole stripes (as
-// frame_hash_buffers), and what is left is moved to the front.  The recurrence is serial: one warp's rate.
-__global__ void __launch_bounds__(32) lizard_frame_stream_hash_kernel(const StreamSeg* seg, u32 n, StreamHashState* st)
+// frame_hash_buffers), and what is left is moved to the front.  The recurrence is serial: one warp's rate.  seg(i, &p, &L)
+// gives segment i; buf is the warp's kHashPiece + 16 bytes of shared memory.
+template <class Seg> __device__ __forceinline__ void stream_hash_segments(Seg seg, u32 n, StreamHashState* st, u8* buf)
 {
-    __shared__ __align__(16) u8 buf[kHashPiece + 16];
     const u32 lane = threadIdx.x;
     u32 v = lane < 4 ? st->v[lane] : 0;
     u32 nb = st->nbuf;
@@ -40,8 +40,9 @@ __global__ void __launch_bounds__(32) lizard_frame_stream_hash_kernel(const Stre
     u64 total = st->total;
     __syncwarp();
     for (u32 i = 0; i < n; ++i) {
-        const u8* p = (const u8*)(size_t)seg[i].src;
-        const u64 L = seg[i].len;
+        const u8* p;
+        u64 L;
+        seg(i, &p, &L);
         total += L;
         for (u64 done = 0; done < L;) {
             const u32 take = (u32)(L - done < kHashPiece - nb ? L - done : kHashPiece - nb);
@@ -75,6 +76,12 @@ __global__ void __launch_bounds__(32) lizard_frame_stream_hash_kernel(const Stre
     if (lane < 4) st->v[lane] = v;
     if (lane < nb) st->buf[lane] = buf[lane];
     if (lane == 0) { st->total = total; st->nbuf = nb; }
+}
+// LizardB200_decompressStream's pieces: a segment list in device memory
+__global__ void __launch_bounds__(32) lizard_frame_stream_hash_kernel(const StreamSeg* seg, u32 n, StreamHashState* st)
+{
+    __shared__ __align__(16) u8 buf[kHashPiece + 16];
+    stream_hash_segments([seg](u32 i, const u8** p, u64* L) { *p = (const u8*)(size_t)seg[i].src; *L = seg[i].len; }, n, st, buf);
 }
 
 }  // namespace lzb

@@ -1047,3 +1047,99 @@ extern "C" void lzb_host_stream_walk(const unsigned char* p, unsigned long long 
     for (lzb::u32 i = 0; i < w.n_recs; ++i) { pos[i] = rec[i].pos; word[i] = rec[i].word; unit[i] = rec[i].unit; }
     summary[0] = w.n_recs; summary[1] = w.stop; summary[2] = w.n_units;
 }
+
+// ---- LizardB200_compressStream* on the host (frame_cstream.h): the shared runs over host memory with the one-lane encoder in
+// place of the kernels, so the CPU tests compare them call for call with the reference's LizardF_compressBegin / Update / flush /
+// End.  Records are written as frame.inl's frame_compress_blocks and the assembly kernel write them (frame_record_payload).
+#include "frame_cstream.h"
+namespace {
+struct HostCStream { lzb::FrameCState st; std::vector<lzb::u8> carry; lzb::StreamHashState h; };
+struct ShimCompressIO {
+    HostCStream* cs;
+    bool ready() { return true; }
+    bool level_ok(int level)
+    {
+        return lzb::level_params(level).parser != lzb::kParserUnsupported || lzb::lp_level(level) || lzb::opt_level(level);
+    }
+    void begin(lzb::u8* dst, const lzb::u8* hdr, lzb::u32 n, size_t bs)
+    {
+        memcpy(dst, hdr, n);
+        lzb::xx_stream_reset(&cs->h);
+        if (cs->carry.size() < bs) cs->carry.resize(bs);
+    }
+    void hash_begin(const lzb::u8*, size_t) {}
+    void hash_end(const lzb::u8* p, size_t n) { lzb::xx_stream_update(&cs->h, p, n); }
+    void hash_abort() {}
+    void carry(size_t at, const lzb::u8* p, size_t n) { memcpy(cs->carry.data() + at, p, n); }
+    size_t compress_carry(lzb::u8* dst, size_t cap, size_t n, int level) { return compress(dst, cap, cs->carry.data(), n, level); }
+    size_t compress(lzb::u8* dst, size_t cap, const lzb::u8* p, size_t n, int level)
+    {
+        const size_t bs = cs->st.block_size;
+        std::vector<lzb::u8> enc(bs + 64);
+        size_t o = 0;
+        for (size_t at = 0; at < n; at += bs) {
+            const lzb::u32 len = (lzb::u32)(n - at < bs ? n - at : bs);
+            const int r = lzb_host_compress(p + at, (int)len, enc.data(), (int)len - 1, level);
+            const lzb::u32 payload = lzb::frame_record_payload(len, r);
+            if (o + 4 + payload > cap) return lzb::ferr(lzb::FE_dstMaxSize_tooSmall);
+            if (len == 1) lzb::frame_one_byte_record(dst + o, level, p[at]);
+            else {
+                lzb::wr_le32(dst + o, r > 0 ? (lzb::u32)r : (len | 0x80000000u));
+                memcpy(dst + o + 4, r > 0 ? enc.data() : p + at, payload);
+            }
+            o += 4 + payload;
+        }
+        return o;
+    }
+    void end_mark(lzb::u8* dst, bool ccksum) { lzb::wr_le32(dst, 0); if (ccksum) lzb::wr_le32(dst + 4, lzb::xx_stream_digest(&cs->h)); }
+};
+}  // namespace
+
+extern "C" void* lzb_host_cstream_new()
+{
+    HostCStream* s = new HostCStream();
+    s->st.reset();
+    lzb::xx_stream_reset(&s->h);
+    return s;
+}
+extern "C" void lzb_host_cstream_free(void* p) { delete (HostCStream*)p; }
+extern "C" size_t lzb_host_cstream_begin(void* p, unsigned char* dst, size_t cap, const LizardF_preferences_t* prefs)
+{
+    HostCStream* s = (HostCStream*)p;
+    ShimCompressIO io{ s };
+    return lzb::frame_cbegin_run(&s->st, io, dst, cap, prefs);
+}
+extern "C" size_t lzb_host_cstream_update(void* p, unsigned char* dst, size_t cap, const unsigned char* src, size_t n)
+{
+    HostCStream* s = (HostCStream*)p;
+    ShimCompressIO io{ s };
+    return lzb::frame_cupdate_run(&s->st, io, dst, cap, src, n);
+}
+extern "C" size_t lzb_host_cstream_flush(void* p, unsigned char* dst, size_t cap)
+{
+    HostCStream* s = (HostCStream*)p;
+    ShimCompressIO io{ s };
+    return lzb::frame_cflush_run(&s->st, io, dst, cap);
+}
+extern "C" size_t lzb_host_cstream_end(void* p, unsigned char* dst, size_t cap)
+{
+    HostCStream* s = (HostCStream*)p;
+    ShimCompressIO io{ s };
+    return lzb::frame_cend_run(&s->st, io, dst, cap);
+}
+// the planning kernel's unit k (cstream_unit): out = source address, length, encoder slot, capacity
+extern "C" void lzb_host_cstream_unit(unsigned k, unsigned long long carry, unsigned long long carry_len, unsigned long long p,
+                                      unsigned long long n, unsigned long long bs, unsigned long long stride, unsigned long long* out)
+{
+    lzb::u64 src, enc;
+    lzb::u32 len, cap;
+    lzb::cstream_unit(k, carry, carry_len, p, n, bs, stride, &src, &len, &enc, &cap);
+    out[0] = src; out[1] = len; out[2] = enc; out[3] = cap;
+}
+// an Update's split of a chunk (frame_cupdate_plan): out = take, whole, rest, carry_block
+extern "C" void lzb_host_cupdate_plan(unsigned long long carry, unsigned long long bs, unsigned auto_flush, unsigned long long n,
+                                      unsigned long long* out)
+{
+    const lzb::CUpdatePlan pl = lzb::frame_cupdate_plan(carry, bs, auto_flush, n);
+    out[0] = pl.take; out[1] = pl.whole; out[2] = pl.rest; out[3] = pl.carry_block;
+}
